@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""Benchmark of the string_grouper hot path on B200 — one JSON line on stdout (rank 0).
+"""Benchmark of the string_grouper hot path on H100 — one JSON line on stdout (rank 0).
 
     python bench.py --gpus 1 --steps 3 --warmup 3
+    python bench.py --gpus 1 --steps 3 --warmup 3 --dump-outputs DIR   # + the last timed step's match list as .npy
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W
     python bench.py --impl reference ...        # the reference's CPU path (oracle port) on this box's cores
@@ -14,7 +15,7 @@ One step = one pass of the hot path: K1 vectorise -> K2 top-n cosine product -> 
   e2e          same metric through string_grouper_b200.StringGrouper(series).fit().get_matches(): host buffers in,
                DataFrame out, H2D / D2H inside the timed region
   roofline     the dominant kernel chain (K2 candidates: pack + block-max filter + tile kernel): bytes it really
-               streams / CUDA-event time, against the measured HBM peak; the bytes of the full Gustavson traversal
+               streams / CUDA-event time, against the H100 SXM data-sheet HBM3 bandwidth; the bytes of the full Gustavson traversal
                (SURVEY.md §8d) are reported beside it as `algorithmic`
   parity       ALL pairs of the step's result against the CPU port's whole-job result (N=1)
   cpu_baseline the CPU port's measured whole job on this box's usable cores (N=1)
@@ -42,7 +43,7 @@ TOP_N, MIN_SIM = 20, 0.8
 
 # ----------------------------------------------------------------------------- clocks
 class ClockSampler:
-    """nvidia-smi sampled every 200 ms while the timed region runs (B200_PROFILING.md recipe).
+    """nvidia-smi sampled every 200 ms while the timed region runs.
 
     start() launches the process early (its NVML initialisation enumerates every GPU of the box and was seen to
     stall rank 0 for 10-15 ms when it fell into a timed step of an 8-GPU run); arm() marks the beginning of the timed
@@ -135,6 +136,8 @@ def run_reference_arm(args, names, sha):
     setup = time.perf_counter() - t0
     job = C.whole_job(names, cores)
     full = job["matrix"]
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, len(names), (job["row"], job["col"], job["score"]))
     ests, walls, last = [], [], None
     for step in range(args.warmup + args.steps):
         t0 = time.perf_counter()
@@ -170,6 +173,26 @@ def run_reference_arm(args, names, sha):
     print(json.dumps(line), flush=True)
 
 
+DUMP_BYTES = 64 << 20       # --dump-outputs: at most this much in all
+DUMP_ROWS = 300_000         # left rows whose pairs are written (a seeded sample when there are more)
+
+
+def dump_outputs(path, n, triples):
+    """The match list of the last timed step as float64 .npy files: match_row, match_col, match_score, sorted by
+    (row, col).  Above DUMP_ROWS left rows only the pairs of a seeded sample of rows that depends on n alone are
+    written, so two builds run with the same arguments write the same rows."""
+    r, c, s = (np.asarray(x) for x in triples)
+    o = np.lexsort((c, r))
+    r, c, s = r[o], c[o], s[o]
+    if n > DUMP_ROWS:
+        keep = (np.random.default_rng(0).random(n) < DUMP_ROWS / n)[r]
+        r, c, s = r[keep], c[keep], s[keep]
+    m = DUMP_BYTES // 24
+    os.makedirs(path, exist_ok=True)
+    for name, a in (("match_row", r), ("match_col", c), ("match_score", s)):
+        np.save(os.path.join(path, name + ".npy"), a[:m].astype(np.float64))
+
+
 def triples_digest(r, c, s):
     """Order-independent digest of a match list (sorted by (row, col) first)."""
     r, c, s = np.asarray(r, dtype=np.int64), np.asarray(c, dtype=np.int64), np.asarray(s, dtype=np.float64)
@@ -179,7 +202,7 @@ def triples_digest(r, c, s):
     return h.hexdigest()[:32]
 
 
-# ----------------------------------------------------------------------------- B200 arm
+# ----------------------------------------------------------------------------- CUDA arm
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -191,7 +214,10 @@ def main():
     ap.add_argument("--no-aux", action="store_true", help="multi-GPU: skip the two-Series sharded-K1 run")
     ap.add_argument("--aux-master", type=int, default=2_000_000)
     ap.add_argument("--aux-duplicates", type=int, default=400_000)
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the match list of the last timed step to DIR/*.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
 
     if os.environ.get("NCCL_DEBUG", "").upper() == "VERSION":
         os.environ["NCCL_DEBUG"] = "WARN"           # keep stdout to the one JSON line
@@ -212,14 +238,14 @@ def main():
     import torch.distributed as dist
 
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a CUDA device (B200); use --impl reference for the CPU arm")
+        raise SystemExit("bench.py needs a CUDA device (H100); use --impl reference for the CPU arm")
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
     sampler = ClockSampler(local_rank)
     if rank == 0:
         sampler.start()          # long before the timed region, see ClockSampler
     if world > 1:
-        os.environ.setdefault("SG_B200_DISTRIBUTED", "1")     # the library shards only when told to (ADVICE r1)
+        os.environ.setdefault("SG_B200_DISTRIBUTED", "1")     # the library shards only when told to
         dist.init_process_group("nccl", device_id=dev)
     import string_grouper_b200 as api
     from string_grouper_b200 import _device as D
@@ -294,6 +320,8 @@ def main():
         dist.all_gather_object(phases_all, phases)
     final_triples = S.host_triples()
     pre_triples = info["M"].host_triples() if world == 1 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, n, final_triples)
 
     # ---- multi-GPU: the gathered result must equal the unsharded one (untimed) ----
     shard_check = None
@@ -399,11 +427,7 @@ def main():
     macs_total = int((df * df).sum().item())
     alg_bytes = 8 * macs_local + 8 * nnz_a_local + 4 * (hi - lo + 1) + 8 * info["k2_nnz_local"] + 4 * (hi - lo + 1)
     k2_ms = float(np.mean(cand_ms))
-    peaks_path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(peaks_path):
-        peak, peak_src = float(json.load(open(peaks_path))["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (measured)"
-    else:
-        peak, peak_src = 6650.0, "B200_PROFILING.md fallback"
+    peak, peak_src = 3350.0, "H100 SXM data sheet HBM3 bandwidth (not measured)"
     # what the launches really read and write: the (row, tile) pairs that survive the block-max test and the postings of
     # their buckets are COUNTED by the tile formulation's kernel on the same input (one untimed run; both formulations
     # apply the same pruning and the same block-max test), the rest follows from the array shapes
@@ -437,32 +461,24 @@ def main():
         streamed["pairs_walked"], streamed["postings_walked"] = pairs_w, post_w
         streamed["note"] = ("pairs / postings counted by sg::tile_candidates_kernel on the same input; upper bounds where "
                             "the kept-feature count is needed (the pruned rows hold fewer features)")
-    traffic = pipe = None
-    tpath = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(tpath) and world == 1:      # the ncu capture is a 1-GPU launch over all rows
-        traffic = json.load(open(tpath)).get("%d" % n)
-    ppath = os.path.join(ROOT, "profiles", "pipe.json")
-    if os.path.exists(ppath) and world == 1:
-        pipe = json.load(open(ppath)).get("%d" % n)
     bytes_real = streamed["total"] if streamed else None
     achieved = (bytes_real / (k2_ms / 1e3) / 1e9) if bytes_real else None
     alg_gbps = alg_bytes / (k2_ms / 1e3) / 1e9
     roofline = {"bound": "hbm", "kernel": "K2 candidates chain: sg::pack_left + sg::tile_filter + sg::tile_candidates"
                 if st.get("kernel") == "tiles" else "sg::cossim_candidates_kernel",
                 "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": (achieved / peak) if achieved else None,
-                "traffic": traffic, "peak_source": peak_src, "kernel_ms": k2_ms,
+                "peak_source": peak_src, "kernel_ms": k2_ms,
                 "kernel_share_of_step": k2_ms / float(np.mean(step_ms)),
                 "streamed": streamed,
                 "note": "achieved/frac = bytes the launches really stream (kernel-counted postings and pairs, array "
-                        "sizes for the rest; served by shared memory / L2, DRAM traffic is `traffic`) / CUDA-event time / "
-                        "measured HBM copy peak.  The kernel is bound by instruction issue and shared-memory atomics, not by "
-                        "HBM: `limiter` holds the ncu pipe utilisation.  `algorithmic` = SURVEY.md §8d bytes of the FULL "
+                        "sizes for the rest; served by shared memory / L2, not all from DRAM) / CUDA-event time / "
+                        "data-sheet HBM bandwidth.  The kernel is bound by instruction issue and shared-memory atomics, not by "
+                        "HBM.  `algorithmic` = SURVEY.md §8d bytes of the FULL "
                         "Gustavson traversal over the same time: an algorithmic gain (exact pruning + block-max skipping), "
                         "not a utilisation.",
                 "algorithmic": {"bytes_per_launch": alg_bytes, "macs_per_launch": macs_local, "macs_total": macs_total,
                                 "GBps_equivalent": alg_gbps, "frac_equivalent": alg_gbps / peak,
                                 "gain_vs_streamed": (alg_bytes / bytes_real) if bytes_real else None},
-                "limiter": pipe,
                 "tile": {k: st.get(k) for k in ("kernel", "tile_w", "warps", "n_tiles", "stage_bytes", "n_candidates",
                                                 "n_refined", "n_above_threshold", "prune", "acc")}}
 
@@ -485,7 +501,7 @@ def main():
             job = C.whole_job(names, cores)
         parity = C.compare(job, pre_triples, final_triples)
         parity["cpu_job"] = "measured by this process" if not job.get("from_cache") else \
-            "measured by `bench.py --impl reference` on this box earlier in this boot (oracle/_cache)"
+            "measured by `bench.py --impl reference` on this machine earlier in this boot (cached in the temp directory)"
         cpu_baseline = {"value": job["pairs"] / job["wall_s"], "unit": UNIT, "cores": job["threads"], "kind": "port",
                         "sample": "the WHOLE job, measured once on this box (%d names, n_blocks=%s, %d OpenMP threads; "
                                   "os.cpu_count() = %s, usable = %d): %.1f s, phases %s"

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""The other BASELINE.json configurations (2, 4, 5; config 3 is bench.py) through the public API — absolute numbers for
-profiles/, not the driver's bench line.
+"""The other BASELINE.json configurations (2, 4, 5; config 3 is bench.py) through the public API — absolute numbers beside
+bench.py's line.
 
     python bench_configs.py --config 2                      # 100k self-match @0.8, 1 GPU
     torchrun --nproc-per-node 8 ... bench_configs.py --config 4   # master 5M x duplicates 1M @0.7, row blocks over 8 GPUs
@@ -142,7 +142,7 @@ def main():
             "pairs_per_s": (len(sg._matches_list) / best),
             "matches": int(len(sg._matches_list)), "k2_macs_rank0": macs, "k2_kernel_ms_rank0": k_ms,
             "k2_algorithmic_GBps_rank0": 8 * macs / (k_ms / 1e3) / 1e9,
-            "k2_frac_of_6570": 8 * macs / (k_ms / 1e3) / 1e9 / 6570.0,
+            "k2_frac_of_h100_datasheet_hbm": 8 * macs / (k_ms / 1e3) / 1e9 / 3350.0,
             "k2_walked_macs_rank0": stats.get("macs_walked"), "prune": stats.get("prune"), "kernel": stats.get("kernel"),
             "select": stats.get("select"),
             "accumulator": stats.get("acc"), "tile_w": stats.get("tile_w"), "warps": stats.get("warps"),

@@ -4,7 +4,7 @@ this box's host cores.  BENCH / TEST INFRASTRUCTURE: this is the only module bes
 __graft_entry__.smoke() that executes anything under oracle/, and only as the baseline / the checker.
 
   whole_job()      ONE measured pass of the reference's match_strings self-match on the whole corpus, phase by
-                   phase (/root/reference/string_grouper/string_grouper.py: __init__ :267, fit :380-431,
+                   phase (string_grouper/string_grouper.py: __init__ :267, fit :380-431,
                    get_matches :443-518), with the true pair count and the match lists for the parity check
   sample_model()   the bounded per-step sample (a 20 000-name fit + two left-row slices against all right rows)
                    and the whole-job estimate it extrapolates to; calibrated against whole_job() by the caller
@@ -14,12 +14,13 @@ import hashlib
 import json
 import os
 import socket
+import tempfile
 import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.abspath(__file__))
-CACHE_DIR = os.path.join(ROOT, "oracle", "_cache")
+# outside the source tree: bench.py must leave the tree untouched (it may be read-only)
+CACHE_DIR = os.path.join(tempfile.gettempdir(), "string_grouper_cpu_jobs")
 TOP_N, MIN_SIM = 20, 0.8
 
 

@@ -1,11 +1,11 @@
 /*
- * sg_b200.h — C ABI of libsg_b200.so, the B200 (sm_100a) implementation of the
+ * sg_b200.h — C ABI of libsg_b200.so, the H100 (sm_90a) implementation of the
  * string_grouper hot path.  Plain pointers and sizes only; no torch types.
  *
  * The reference (Bergvca/string_grouper @ 270044e9, pure Python) has no FFI of
  * its own: its hot path calls scikit-learn and sparse_dot_topn.  Every entry
  * point below names the reference interface it replaces as
- * /root/reference/string_grouper/string_grouper.py:<line> ("sg.py:<line>").
+ * string_grouper/string_grouper.py:<line> ("sg.py:<line>").
  *
  * Conventions
  *   - every pointer marked [dev] is device memory owned by the caller

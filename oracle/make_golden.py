@@ -1,11 +1,11 @@
 """TEST INFRASTRUCTURE — golden-vector generator.
 
-Runs the UNMODIFIED reference (/root/reference/string_grouper) — with the C oracle standing in for
-the absent `sparse_dot_topn` wheel (oracle/standin/) — on the reference's own fixtures, the tutorial
-data and two seeded synthetic corpora, and writes the answers under tests/golden/.  /root/reference
-does not exist on the GPU box, hence the committed fixtures.
+Runs the UNMODIFIED reference (a checkout of Bergvca/string_grouper) — with the C oracle standing in
+for the absent `sparse_dot_topn` wheel (oracle/standin/) — on the reference's own fixtures, the tutorial
+data and two seeded synthetic corpora, and writes the answers under tests/golden/.  The tests replay
+the committed fixtures, so they do not need the reference checkout.
 
-    python oracle/make_golden.py        # in the build container only
+    python oracle/make_golden.py /path/to/string_grouper_checkout
 """
 import json
 import os
@@ -17,7 +17,8 @@ import pandas as pd
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 sys.path.insert(0, os.path.join(HERE, "standin"))
-sys.path.insert(0, "/root/reference")
+REFERENCE = os.path.abspath(sys.argv[1] if len(sys.argv) > 1 else os.environ.get("STRING_GROUPER_SRC", "."))
+sys.path.insert(0, REFERENCE)
 sys.path.insert(0, ROOT)
 
 from string_grouper import (StringGrouper, compute_pairwise_similarities, group_similar_strings,  # noqa: E402
@@ -80,7 +81,7 @@ def cases():
     """name -> (callable description for the test, result).  Every entry is replayed by
     tests/test_golden_api.py through string_grouper_b200 with the same arguments."""
     out = {}
-    acc = pd.read_csv("/root/reference/tutorials/accounts.csv")
+    acc = pd.read_csv(os.path.join(REFERENCE, "tutorials", "accounts.csv"))
     df, df2 = customers()
     names, ids = df['Customer Name'], df['Customer ID']
     names2, ids2 = df2['Customer Name'], df2['Customer ID']
@@ -229,6 +230,6 @@ if __name__ == "__main__":
         json.dump(c, f, indent=1, sort_keys=True)
     arr = synthetic()
     np.savez_compressed(os.path.join(OUT, "synthetic.npz"), **arr)
-    acc = pd.read_csv("/root/reference/tutorials/accounts.csv")
+    acc = pd.read_csv(os.path.join(REFERENCE, "tutorials", "accounts.csv"))
     acc.to_csv(os.path.join(OUT, "accounts_input.csv"), index=False)   # 14-row tutorial input, data not code
     print("wrote %d api cases, %d arrays" % (len(c), len(arr)))

@@ -4,7 +4,7 @@ CPU restatement of the reference hot path, function by function, on top of the
 real scikit-learn / scipy (both are the reference's own dependencies and are
 installed on every box of this image) and the C oracle for `sparse_dot_topn`.
 
-Citations are /root/reference/string_grouper/string_grouper.py:<line>.
+Citations are string_grouper/string_grouper.py:<line>.
 """
 import re
 from unicodedata import normalize

@@ -2,7 +2,7 @@
 
 Python face of the C oracle (`oracle/sdt_oracle.c`): the two callables the
 reference imports from the absent third-party package `sparse_dot_topn`
-(/root/reference/string_grouper/string_grouper.py:12), with the keyword
+(string_grouper/string_grouper.py:12), with the keyword
 signatures the reference uses at :725-732, :737-743 and :746.
 
 `oracle/standin/sparse_dot_topn/` re-exports these under the upstream module

@@ -3,13 +3,13 @@
  *
  * CPU restatement (plain C + OpenMP) of the two operators that the reference
  * hot path delegates to the third-party package `sparse_dot_topn` (>=1.1.0,
- * un-pinned: /root/reference/pyproject.toml:30, /root/reference/setup.py:28;
- * the wheel is neither vendored under /root/reference nor installable here):
+ * un-pinned: pyproject.toml:30, setup.py:28 of the reference;
+ * the wheel is not vendored with the reference):
  *
  *   sp_matmul_topn(A, B, top_n, threshold, sort, n_threads)
- *       call sites: /root/reference/string_grouper/string_grouper.py:725-732, :737-743
+ *       call sites: string_grouper/string_grouper.py:725-732, :737-743
  *   zip_sp_matmul_topn(top_n, C_mats)
- *       call site:  /root/reference/string_grouper/string_grouper.py:746
+ *       call site:  string_grouper/string_grouper.py:746
  *
  * Published algorithm restated here (SURVEY.md Appendix A.3 / A.4):
  *   per output row i, Gustavson row-wise SpGEMM into a dense accumulator

@@ -1,5 +1,5 @@
 """TEST INFRASTRUCTURE — stand-in for the absent `sparse_dot_topn` wheel so the
-UNMODIFIED reference (/root/reference/string_grouper/string_grouper.py:12) can be
+UNMODIFIED reference (string_grouper/string_grouper.py:12) can be
 imported by oracle/make_golden.py and the reference-suite pin test."""
 import os
 import sys

@@ -21,7 +21,9 @@ TRANSFER_BYTES = {"d2h": 0, "h2d": 0}      # bytes moved by the bulk copies (ben
 
 DEFAULT_TILE_W = int(os.environ.get("SG_B200_TILE_W", "0"))         # 0: 256 (u16) columns per tile, 128 for large right matrices
 DEFAULT_WARPS = int(os.environ.get("SG_B200_WARPS", "8"))           # 8 warps x 5 CTAs at 48 registers (no spills)
-GROUP_BYTES = int(os.environ.get("SG_B200_GROUP_MB", "12")) << 20   # posting bytes one column-tile group may hold
+# posting bytes one column-tile group may hold: a group's buckets should stay resident in H100's 50 MB L2 next to the
+# rest of the working set (663k rows on H100: 6 MB groups 43.4-44.0 ms for the candidates kernel, 12 MB 45.5-46.2, 24 MB 49.4)
+GROUP_BYTES = int(os.environ.get("SG_B200_GROUP_MB", "6")) << 20
 CAND_MARGIN = 1.5e-3   # candidates: fp16 posting weights (<= 4.9e-4) + fp32 accumulation; all are re-scored exactly
 U16_MARGIN_PER_FEATURE = 2e-5   # 1/32768 fixed-point accumulator tile: one rounding of <= 2^-16 per added product
 # Exact threshold pruning (csrc/sg_prune.cu): the most expensive heavy features of a left row are skipped while
@@ -36,8 +38,8 @@ OPTIMISTIC_PAIRS = float(os.environ.get("SG_B200_OPTIMISTIC_PAIRS", "5e11"))
 REFINE = os.environ.get("SG_B200_REFINE", "1") != "0"      # grouped per-candidate bound before the exact re-score
 # K2 formulation: "row" (the default) = one warp per left row over L2-resident posting buckets (csrc/sg_cossim.cu; also
 # the general path: negative values, norms above 1, near-zero thresholds); "tiles" = right tiles staged through TMA into
-# shared memory (csrc/sg_tiles.cu), for L2-normalised non-negative operands.  Measured on B200 at 663k rows the row kernel
-# is the faster one (DESIGN.md §4: both are bound by instruction issue at ~340 warp instructions per (row, tile) pair).
+# shared memory (csrc/sg_tiles.cu), for L2-normalised non-negative operands.  Measured on H100 at 663k rows the row kernel
+# is the faster one (65 vs 80 ms per step, DESIGN.md §4).
 K2_KERNEL = os.environ.get("SG_B200_KERNEL", "row").lower()
 TILE_MARGIN = 2e-5               # fp32 arithmetic of thresholds / norms and the f64 -> f32 copy of the values
 TILE_MARGIN_PER_FEATURE = 3.1e-5  # a_q * w_q / 2^30 vs a * w: both weights rounded to nearest 2^-15 (<= 2^-15 + 2^-32)
@@ -56,7 +58,7 @@ def torch():
 def require_cuda():
     t = torch()
     if not t.cuda.is_available():
-        raise _lib.SgB200Error("string_grouper_b200 needs a CUDA device (B200, sm_100a); there is no CPU fallback "
+        raise _lib.SgB200Error("string_grouper_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback "
                                "for the hot path")
     _lib.load()
     return t
@@ -121,7 +123,7 @@ class DeviceCSR:
     """CSR matrix resident in HBM: indptr int64, indices int32, val (matrix dtype), val32 (fp32 copy).
 
     Quacks like the scipy matrices StringGrouper._get_tf_idf_matrices returns
-    (/root/reference/string_grouper/string_grouper.py:685-697): `.shape`,
+    (string_grouper/string_grouper.py:685-697): `.shape`,
     `.toarray()`, `.indptr` ... are served from a lazily materialised scipy
     copy, so reference-style tests and user code keep working.
     """
@@ -407,9 +409,9 @@ def pick_tile(n_right, tile_w=None, warps=None, acc_bytes=4, n_left=None):
     point): narrow tiles make the block-max test skip most (row, tile) pairs, and the test itself costs a
     fraction of an instruction per pair."""
     warps = int(warps or DEFAULT_WARPS)
-    # measured on B200 (profiles/r2_notes.md): 128-column tiles win from a few 10^5 right rows on (the block-max test
-    # skips more, 34.5 vs 38.0 ms at 663k), 256-column tiles below (1.4 vs 1.8 ms at 100k: fewer directory entries)
-    # (the finer directory costs ~0.6 ms more to build: not worth it for a small block of left rows, e.g. one of 8 shards)
+    # 128-column tiles from a few 10^5 right rows on (the block-max test skips more; 663k on H100, 12 MB groups: 45.5-45.9 ms for the
+    # candidates kernel vs 46.1-46.9 at 256 columns), 256-column tiles below (fewer directory entries to build, which
+    # is not worth it for a small block of left rows, e.g. one of 8 shards)
     many_left = n_left is None or int(n_left) >= 150_000
     auto_w = 128 if (acc_bytes == 4 or (int(n_right) >= 400_000 and many_left)) else 256
     tile_w = int(tile_w or DEFAULT_TILE_W) or auto_w
@@ -691,7 +693,7 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
             n_cand = timed_launch(perm_chunk, row_begin, row_begin + (hi - lo), cand_row, cand_col, cap, cand_part)
             if n_cand <= cap:
                 break
-            if n_cand * 24 > 96 * 2**30:
+            if n_cand * 24 > t.cuda.get_device_properties(dev).total_memory // 2:
                 raise OverflowError("%d candidate pairs above the threshold do not fit the candidate buffer; "
                                     "raise min_similarity or split the input" % n_cand)
             cap = n_cand

@@ -1,6 +1,6 @@
 """Multi-GPU sharding of the hot path: one process per GPU (torchrun), torch.distributed for plumbing.
 
-The block loop of StringGrouper._build_matches (/root/reference/string_grouper/string_grouper.py:734-750)
+The block loop of StringGrouper._build_matches (string_grouper/string_grouper.py:734-750)
 is data-parallel over LEFT row blocks (their results are only `vstack`ed, :750); right blocks need a
 per-row merge (:746), so the right side is never split across GPUs.  Rank g owns the left rows
 `define_chunks(n_left, world)[g]` (same ceil-sized chunking as :721-722), runs K2 on them against the

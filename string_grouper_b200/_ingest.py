@@ -1,7 +1,7 @@
 """Host side of the analyzer: pandas Series -> (uint8 bytes, int64 offsets) for the device vectoriser.
 
 The device kernel (csrc/sg_tfidf.cu) implements the analyzer of the reference
-(/root/reference/string_grouper/string_grouper.py:365-378) for ASCII text with
+(string_grouper/string_grouper.py:365-378) for ASCII text with
 the default regex.  This module does what has to stay in Python:
 
   * validation (string_grouper.py:351-352, :988-995): every element must be a `str`;

@@ -2,7 +2,7 @@
 
 The product path has no CPU fallback: if the shared library is missing or a
 CUDA device is absent, the callers raise.  Build with
-`python -c "import __graft_entry__ as g; g.build()"` (nvcc, sm_100a).
+`python -c "import __graft_entry__ as g; g.build()"` (nvcc, sm_90a).
 """
 import ctypes
 import os

@@ -1,4 +1,4 @@
-// Shared helpers for the libsg_b200.so translation units (sm_100a only).
+// Shared helpers for the libsg_b200.so translation units (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -7,8 +7,8 @@
 
 #include "../../include/sg_b200.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "libsg_b200 is written for sm_100a (B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 900)
+#error "libsg_b200 needs sm_90a or newer (TMA bulk copies, mbarrier transaction counts)"
 #endif
 
 namespace sg {

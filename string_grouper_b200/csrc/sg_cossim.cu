@@ -1,7 +1,7 @@
-// K2 — blocked CSR x CSR^T, thresholded, top-n per left row, for sm_100a.
+// K2 — blocked CSR x CSR^T, thresholded, top-n per left row, for sm_90a.
 //
 // Replaces StringGrouper._build_matches
-// (/root/reference/string_grouper/string_grouper.py:709-752): the per block
+// (string_grouper/string_grouper.py:709-752): the per block
 // pair sp_matmul_topn products (:737-743), the zip over right blocks (:746)
 // and the vstack over left blocks (:750).  See DESIGN.md §K2 for the layout.
 //
@@ -94,8 +94,7 @@ constexpr int LONG_BUCKET = 64;  // buckets from this length on are streamed by 
 #endif
 #ifndef SG_FILTER_MLP
 #define SG_FILTER_MLP 1          // block-maxima loads in flight per lane in the block-max test
-// Measured on B200, 663k rows (profiles/r2_notes.md): 1/1 34.3 ms; walk 2 / filter 4: 38.0; 4 / 8: 41.5; 1 / 8: 38.8; 4 / 1: 36.6.
-// With 40 resident warps the load latency is already covered; the extra registers / predicated work only cost issue slots.
+// With 40 resident warps the load latency is covered; more loads in flight cost registers and issue slots.
 #endif
 
 // Resident CTAs per SM the register allocation is made for (the accumulator tiles are small, registers decide):

@@ -1,6 +1,6 @@
-// Device string gather for get_matches (SURVEY.md §8f row 1), for sm_100a.
+// Device string gather for get_matches (SURVEY.md §8f row 1), for sm_90a.
 //
-// StringGrouper.get_matches (/root/reference/string_grouper/string_grouper.py:455-468) gathers the left and
+// StringGrouper.get_matches (string_grouper/string_grouper.py:455-468) gathers the left and
 // right strings of every match by position (`Series.iloc[matches_list.master_side]`).  The packed strings are
 // already in HBM for K1 and the match positions are there after K4, so the gather runs on the device and one
 // contiguous (offsets, bytes) pair per side goes back to the host, where it is wrapped as an Arrow string array

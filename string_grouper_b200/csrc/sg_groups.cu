@@ -1,7 +1,7 @@
-// Group representatives on the device, for sm_100a  (SURVEY.md §8f row 2).
+// Group representatives on the device, for sm_90a  (SURVEY.md §8f row 2).
 //
 // Replaces the arithmetic of StringGrouper._deduplicate
-// (/root/reference/string_grouper/string_grouper.py:851-904): weakly connected components of the match
+// (string_grouper/string_grouper.py:851-904): weakly connected components of the match
 // graph (scipy.sparse.csgraph.connected_components, :863), per-row similarity sums (:875-881) and the
 // per-group choice of the representative: the first member ('first', :872-873) or the first member with
 // the largest similarity sum ('centroid', :885-886, idxmax).

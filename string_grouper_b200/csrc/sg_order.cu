@@ -1,7 +1,7 @@
-// Row ordering by heavy-feature signature, for sm_100a.
+// Row ordering by heavy-feature signature, for sm_90a.
 //
 // No reference counterpart: this is layout work for K2 (the reference's block loop,
-// /root/reference/string_grouper/string_grouper.py:734-750, takes rows in input order).  The product
+// string_grouper/string_grouper.py:734-750, takes rows in input order).  The product
 // C = A * B^T is invariant under row permutations of A and of B, so both sides are processed in an
 // order that puts rows sharing the same frequent n-grams next to each other:
 //   * left tiles of R consecutive rows then share most of their heavy features, so one posting read

@@ -1,6 +1,6 @@
-// Exact threshold pruning of the left operand of K2, for sm_100a (SURVEY.md §8f row 4).
+// Exact threshold pruning of the left operand of K2, for sm_90a (SURVEY.md §8f row 4).
 //
-// No reference counterpart: sp_matmul_topn (call sites /root/reference/string_grouper/string_grouper.py:725-743)
+// No reference counterpart: sp_matmul_topn (call sites string_grouper/string_grouper.py:725-743)
 // walks every posting of every feature of a left row.  With x = x_P + x_S (P = a set of the row's features)
 //
 //     x . y  =  x_P . y + x_S . y  <=  |x_P| |y| + x_S . y            (Cauchy-Schwarz)
@@ -25,7 +25,7 @@
 // (fp16, rounded up, 32 bytes = one sector per row); sg_rescore_refined re-tests every candidate (row i, column j)
 // with  partial score > threshold(i) - sum_g |x_P,g(i)| |y_H,g(j)|  before it reads the right row.  Candidates per
 // left row on the 663k benchmark (sample): tile-wide bound 501, 8 groups of 8 ranks 85, this grouping 45, pairs
-// above the threshold 42 (profiles/r2_notes.md).
+// above the threshold 42 (tests/gpu_bound_stats.py).
 #include <cuda_fp16.h>
 
 #include "sg_common.cuh"

@@ -1,6 +1,6 @@
-// K2 tail — segmented per-row top-n selection, for sm_100a.
+// K2 tail — segmented per-row top-n selection, for sm_90a.
 //
-// The heap of sp_matmul_topn (call sites /root/reference/string_grouper/string_grouper.py:725-743; SURVEY.md Appendix
+// The heap of sp_matmul_topn (call sites string_grouper/string_grouper.py:725-743; SURVEY.md Appendix
 // A.3): per left row keep the `top_n` largest scores strictly above the threshold, emit them value-descending
 // (sort=True).  sg_topn_select (sg_cossim.cu) does this with three global radix sorts over all survivors; here the
 // survivors are bucketed by row (the exact re-score has already counted them per row), and every row is ranked on

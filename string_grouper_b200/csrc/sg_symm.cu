@@ -1,7 +1,7 @@
-// K4 — self-match post-processing on the device, for sm_100a.
+// K4 — self-match post-processing on the device, for sm_90a.
 //
 // Replaces the LIL round trip of StringGrouper.fit
-// (/root/reference/string_grouper/string_grouper.py:419-427) with
+// (string_grouper/string_grouper.py:419-427) with
 // _fix_diagonal (:955-958: M[r,r] = 1 for every r) and _symmetrize_matrix
 // (:961-964: M[c,r] = M[r,c] for every stored (r,c)), followed by tocsr()
 // which orders every row by ascending column.

@@ -1,7 +1,7 @@
-// K1 — character n-gram TF-IDF with the CSR emitted directly in HBM, for sm_100a.
+// K1 — character n-gram TF-IDF with the CSR emitted directly in HBM, for sm_90a.
 //
 // Replaces, for ASCII input (the Python host normalises the rare non-ASCII rows
-// first, exactly /root/reference/string_grouper/string_grouper.py:372-375):
+// first, exactly string_grouper/string_grouper.py:372-375):
 //   StringGrouper.n_grams                         string_grouper.py:365-378
 //   TfidfVectorizer(min_df=1, analyzer=n_grams).fit / .transform
 //                                                 string_grouper.py:305-308, :685-707

@@ -1,4 +1,4 @@
-// K1, general form — character n-gram TF-IDF with 64-bit keys and a sort-based vocabulary, for sm_100a.
+// K1, general form — character n-gram TF-IDF with 64-bit keys and a sort-based vocabulary, for sm_90a.
 //
 // Same reference functions as sg_tfidf.cu (StringGrouper.n_grams string_grouper.py:365-378; TfidfVectorizer fit /
 // transform :305-308, :685-707), for everything its dense 2^(7n) key table cannot hold: ngram_size >= 4 and text

@@ -1,7 +1,7 @@
-// K2, tile-centric formulation for sm_100a: right-matrix row segments staged through TMA into shared memory.
+// K2, tile-centric formulation for sm_90a: right-matrix row segments staged through TMA into shared memory.
 //
 // Replaces the block loop of StringGrouper._build_matches
-// (/root/reference/string_grouper/string_grouper.py:734-750: `Bs` = row blocks of the right matrix, one
+// (string_grouper/string_grouper.py:734-750: `Bs` = row blocks of the right matrix, one
 // sp_matmul_topn per (left block, right block) pair, :737-743) for L2-normalised non-negative matrices
 // (the K1 output).  Where the reference slices ~4000-row right blocks so that the accumulators of
 // sparse_dot_topn stay cache-resident (:387-389), this kernel takes 256-row right blocks ("column tiles"

@@ -1,5 +1,5 @@
 """CUDA stand-ins for the two callables the reference imports from `sparse_dot_topn`
-(/root/reference/string_grouper/string_grouper.py:12), with the keyword usage of its call sites (:725-732, :737-743, :746):
+(string_grouper/string_grouper.py:12), with the keyword usage of its call sites (:725-732, :737-743, :746):
 
     from string_grouper_b200.sparse_dot_topn_compat import sp_matmul_topn, zip_sp_matmul_topn
 

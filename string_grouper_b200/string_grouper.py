@@ -1,7 +1,7 @@
-"""Host-side mirror of the reference interface for the hot path, calling the sm_100a kernels.
+"""Host-side mirror of the reference interface for the hot path, calling the sm_90a kernels.
 
 Drop-in for `string_grouper.string_grouper` of Bergvca/string_grouper @ 270044e9
-(/root/reference/string_grouper/string_grouper.py, cited below as "ref:<line>"):
+(string_grouper/string_grouper.py, cited below as "ref:<line>"):
 same public names, keyword arguments, column labels, exceptions and result
 ordering.  What differs is where the arithmetic runs:
 
