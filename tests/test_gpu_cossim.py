@@ -3,6 +3,7 @@ through the C ABI, against the CPU oracle on the same seeded inputs."""
 import numpy as np
 import pytest
 
+from exact_topn import assert_same, exact_topn
 from parity import compare_triples, csr_triples, row_cutoffs
 from synth_corpus import make_names
 
@@ -47,6 +48,8 @@ def test_self_match_matches_oracle(n, top_n, thr, dtype, kernel):
     st = compare_triples(csr_triples(ref), (gr, gc, gs), n, thr, cutoff_row=cut, label="self %d" % n)
     assert st["common"] + st["boundary_ties"] >= n * 0.95   # at least the diagonal (ties may swap it)
     assert got.max_row == int(np.diff(ref.indptr).max())
+    # bit for bit the exact reference (tests/exact_topn.py), ties and scores at the threshold included
+    assert_same((gr, gc, gs, got.max_row), exact_topn(m, m, top_n, thr), "self %d exact" % n)
     # entries of a row come out by descending score (sort=True, string_grouper.py:730)
     same_row = gr[1:] == gr[:-1]
     assert np.all(gs[1:][same_row] <= gs[:-1][same_row])

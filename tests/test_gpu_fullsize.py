@@ -59,6 +59,25 @@ def test_full_size_kernels_and_pruning_levels_agree(fitted):
             assert np.array_equal(x, y)
 
 
+def test_full_size_exact_on_sampled_rows(fitted):
+    """663k: 2 000 sampled rows of the default product against the exact reference (tests/exact_topn.py), bit for bit
+    with no exemption; at this size the row kernel uses 128-column tiles walked in column-tile groups."""
+    from exact_topn import assert_same, exact_topn
+    from string_grouper_b200 import _device as D
+    names, sg = fitted
+    A, _ = sg._get_tf_idf_matrices()
+    st = {}
+    got = D.cossim_topn(A, A, 20, 0.8, stats=st)
+    assert st["kernel"] == "row" and st["acc"] == "u16" and st["select"] == "rows" and "n_refined" in st
+    assert st["tile_w"] == 128 and st["tiles_per_group"] < st["n_tiles"]        # several column-tile groups
+    host = A.to_scipy()
+    rows = np.sort(np.random.default_rng(8).choice(N, 2000, replace=False))
+    r, c, s, _ = exact_topn(host[rows], host, 20, 0.8, block_rows=128)
+    gr, gc, gs = got.host_triples()
+    sel = np.isin(gr, rows)
+    assert_same((gr[sel], gc[sel], gs[sel]), (rows[r], c, s), "663k, sampled rows")
+
+
 def test_full_size_all_pairs_equal_cpu_port(fitted):
     """BASELINE.json's headline configuration, EVERY pair: the whole 663k product on the CPU port with the reference's
     own block split (string_grouper.py:387-394 -> n_blocks (1, 166)), then fix-diagonal / symmetrise, against the CUDA
