@@ -216,6 +216,11 @@ int sg_tile_bounds(int64_t n_right, const int32_t *perm /*[dev] position -> row,
  * `row_queue` [dev] (zeroed) is the dynamic work queue over (column-tile group, left row) items,
  * groups outermost, `tiles_per_group` column tiles per group (a multiple of 64, sized by the caller so that one
  * group's posting buckets stay L2-resident).
+ * Triangle of a self-match: with `diag_rank` (per left row id: the row's position in the processing order of the
+ * right rows, which must be the same matrix) row i only reports the columns at positions >= diag_rank[i], so every
+ * unordered pair {i, j} is reported once (the pair (i, i) too); sg_rescore's `mirror_count` restores the other half.
+ * `group_items` [dev] sg_num_tiles()/tiles_per_group + 1 entries (rounded up) is scratch for the work items of the
+ * triangle, required with diag_rank.
  */
 #define SG_ACC_F32 0
 #define SG_ACC_U16 1 /* 1/32768 fixed point: caller adds 2e-5 per kept feature to the margin; weights >= 0, scores < 2 */
@@ -232,7 +237,9 @@ int sg_cossim_candidates(const int64_t *a_indptr /*[dev]*/, const int32_t *a_len
                          float cand_threshold, const float *cand_threshold_row /*[dev] per row id, or NULL*/,
                          const float *pruned_norm_row /*[dev] per row id, or NULL*/,
                          const float *tile_bound /*[dev] sg_num_tiles_padded() entries, zero padded*/,
-                         int64_t tiles_per_group, int32_t *cand_row /*[dev] cap*/,
+                         int64_t tiles_per_group, const int32_t *diag_rank /*[dev] per left row id, or NULL*/,
+                         unsigned long long *group_items /*[dev] scratch, with diag_rank*/,
+                         int32_t *cand_row /*[dev] cap*/,
                          int32_t *cand_col /*[dev] cap*/,
                          float *cand_partial /*[dev] cap or NULL: the candidate's partial score over the kept features
                                                as accumulated (input of sg_rescore_refined)*/,
@@ -258,6 +265,11 @@ int sg_cossim_candidates(const int64_t *a_indptr /*[dev]*/, const int32_t *a_len
  *   sg_tiles_candidates  persistent CTAs over (tile, rank segment) items from `queue` [dev, zeroed]; reports
  *                        (row, col) in original ids; cand_count as in sg_cossim_candidates; `walk_stats`
  *                        [dev, 2 x u64, optional]: (row, tile) pairs taken and postings added
+ * Triangle of a self-match as in sg_cossim_candidates: with `diag_rank` (per left row id; needs `perm`) the filter
+ * sets no bit for a tile below the one holding diag_rank[row] and writes the smallest such tile of every 32 ranks
+ * to `diag_tile_min` [dev, mask_stride / 32 entries]; sg_tiles_candidates (same diag_rank and diag_tile_min, which
+ * it overwrites) skips the (tile, segment) items below all rows of the segment and drops the columns before
+ * diag_rank[row].
  * Limits: n_cols <= sg_tiles_max_cols(); one tile's blob must fit shared memory (else SG_ERR_UNSUPPORTED and
  * the caller falls back to sg_cossim_candidates).
  * ------------------------------------------------------------------------- */
@@ -281,13 +293,18 @@ int sg_tiles_pack_left(int64_t n_ranks, const int32_t *perm /*[dev] or NULL*/, i
 int64_t sg_tiles_mask_words(int64_t n_right);
 int sg_tiles_filter(int64_t n_ranks, const void *rowinfo /*[dev]*/, const void *lpack /*[dev]*/,
                     const void *bucket_maxw /*[dev]*/, int64_t n_right, const float *tile_bound /*[dev]*/,
+                    const int32_t *perm /*[dev] as given to sg_tiles_pack_left, or NULL*/,
+                    const int32_t *diag_rank /*[dev] per row id, or NULL*/,
+                    uint32_t *diag_tile_min /*[dev] mask_stride/32, with diag_rank*/,
                     uint32_t *mask /*[dev] words*mask_stride*/, int64_t mask_stride, void *stream);
 size_t sg_tiles_smem_bytes(int stage_bytes, int warps_per_cta);
 int sg_tiles_candidates(const int32_t *perm_a /*[dev] or NULL*/, int64_t n_ranks, int64_t row_begin,
                         const void *rowinfo /*[dev]*/, const void *lpack /*[dev]*/, const uint32_t *mask /*[dev]*/,
                         int64_t mask_stride, const void *tile_desc /*[dev]*/, const void *blob /*[dev]*/,
                         int64_t n_right, int64_t n_cols, const float *tile_bound /*[dev]*/,
-                        const int32_t *perm_b /*[dev] or NULL*/, int stage_bytes /* maxima[0] */,
+                        const int32_t *perm_b /*[dev] or NULL*/, const int32_t *diag_rank /*[dev] or NULL*/,
+                        uint32_t *diag_tile_min /*[dev] from sg_tiles_filter, with diag_rank*/,
+                        int stage_bytes /* maxima[0] */,
                         int32_t *cand_row /*[dev] cap*/, int32_t *cand_col /*[dev] cap*/, int64_t cand_cap,
                         unsigned long long *cand_count /*[dev] 1*/, unsigned long long *queue /*[dev] 1*/,
                         unsigned long long *walk_stats /*[dev] 2 or NULL*/, int warps_per_cta, void *stream);
@@ -300,12 +317,17 @@ int sg_tiles_candidates(const int32_t *perm_a /*[dev] or NULL*/, int64_t n_ranks
  * path bit for bit.  With `keep_count` == NULL score_out[i] is the score of candidate i.  Otherwise only the
  * candidates scoring strictly above `keep_threshold` (sg.py:729/:740) are kept, compacted in no particular
  * order into (keep_row, keep_col, score_out), and *keep_count [dev] (zeroed by the caller) receives their number.
+ * Mirror (`mirror_count` [dev, zeroed] or NULL; needs keep_count): the candidates are the triangle of a self-match
+ * (sg_cossim_candidates with diag_rank, left = right matrix); every kept (r, c) with r != c is also written as (c, r)
+ * with the same score (bit-equal: the merge adds the same products in the same order), counted in *keep_count
+ * and in *mirror_count, and row_cnt counts it for row c.  The keep buffers then need 2 * n_cand entries.
  */
 int sg_rescore(int64_t n_cand, const int32_t *cand_row, const int32_t *cand_col,
                const int64_t *a_indptr, const int32_t *a_indices, const void *a_val,
                const int64_t *b_indptr, const int32_t *b_indices, const void *b_val, int dtype,
                double *score_out /*[dev] n_cand*/, double keep_threshold, int32_t *keep_row /*[dev] n_cand or NULL*/,
                int32_t *keep_col /*[dev] n_cand or NULL*/, unsigned long long *keep_count /*[dev] 1 or NULL*/,
+               unsigned long long *mirror_count /*[dev] 1 or NULL*/,
                int32_t *row_cnt /*[dev] per left row - row_begin, zeroed by the caller, or NULL: += kept per row*/,
                int64_t row_begin, void *stream);
 /* sg_rescore behind the per-candidate grouped bound of csrc/sg_prune.cu: candidate i = (r, c) is only scored when
@@ -313,7 +335,7 @@ int sg_rescore(int64_t n_cand, const int32_t *cand_row, const int32_t *cand_col,
  * (partial score from sg_cossim_candidates, group norms from sg_prune_rows / sg_heavy_norms, row_threshold =
  * sg_prune_rows' out_threshold): the others cannot reach the threshold and their right rows are never read.  Same
  * kept set and scores as sg_rescore on the same candidates.  *refined_count [dev] (zeroed, or NULL) += candidates that
- * were scored.  keep_count / keep_row / keep_col are required. */
+ * were scored.  keep_count / keep_row / keep_col are required; `mirror_count` as in sg_rescore. */
 int sg_rescore_refined(int64_t n_cand, const int32_t *cand_row, const int32_t *cand_col,
                        const float *cand_partial /*[dev] n_cand*/,
                        const void *left_group_norms /*[dev] fp16[16] per left row id*/,
@@ -324,6 +346,7 @@ int sg_rescore_refined(int64_t n_cand, const int32_t *cand_row, const int32_t *c
                        double *score_out /*[dev] n_cand*/, double keep_threshold, int32_t *keep_row /*[dev] n_cand*/,
                        int32_t *keep_col /*[dev] n_cand*/, unsigned long long *keep_count /*[dev] 1*/,
                        unsigned long long *refined_count /*[dev] 1 or NULL*/,
+                       unsigned long long *mirror_count /*[dev] 1 or NULL*/,
                        int32_t *row_cnt /*[dev] or NULL*/, int64_t row_begin, void *stream);
 
 /*

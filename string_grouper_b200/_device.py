@@ -533,16 +533,25 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
         hrank, perm_b, _, bucket_dir, bucket_maxw, post, T, tile_bound = right_side(B, tile_w)
         # column tiles per work group (a multiple of 64): the group's posting buckets should stay L2-resident
         tiles_per_group = max(64, int(GROUP_BYTES // max(4 * B.nnz / T, 1)) // 64 * 64)
-    if A is B and row_begin == 0 and row_end == n_left:
-        perm_a = perm_b
+    # Self-match over all rows: the score is symmetric, so only the triangle of pairs (i, j) with j at or after i in
+    # the common processing order is computed (diag_rank = each row's position in it) and the re-score mirrors every
+    # kept pair.  Row ranges (shards) and two matrices keep the full product.
+    triangle = A is B and row_begin == 0 and row_end == n_left
+    if triangle:
+        perm_a, diag_rank = perm_b, right_order(B)[2]
     else:
         perm_a, _ = row_order(A, hrank, row_begin, row_end, want_rank=False)
+        diag_rank = None
     mark(stats, "right_side")
     c_count = ctypes.c_void_p(counters.data_ptr())
     c_queue = ctypes.c_void_p(counters.data_ptr() + 8)
     c_walk = ctypes.c_void_p(counters.data_ptr() + 16)
+    c_mirror = ctypes.c_void_p(counters.data_ptr() + 24) if triangle else None
     dummy = _empty(1, t.int32, dev)
     pruned = {}
+    group_items = None
+    if triangle and not use_tiles:
+        group_items = _empty(-(-T // tiles_per_group) + 1, t.int64, dev)
 
     def launch_tiles(perm, n, row_buf, col_buf, capacity):
         """pack the pruned rows of `perm`, block-max filter -> survivor bits, tile kernel"""
@@ -550,16 +559,18 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
         stride = (n + 31) // 32 * 32
         rowinfo = _empty(4 * stride, t.int32, dev)
         mask = _empty(mask_words * stride, t.int32, dev)
+        diag_tile_min = _empty(stride // 32, t.int32, dev) if triangle else None
         counters.zero_()
         _lib.check(L.sg_tiles_pack_left(n, _ptr(perm), 0, _ptr(A.d_indptr), _ptr(l_len), _ptr(l_idx), _ptr(l_val),
                                         _ptr(l_thr), _ptr(l_xp), max(B.norm_bound, 1.0), _ptr(lpack), _ptr(rowinfo),
                                         _stream()))
         _lib.check(L.sg_tiles_filter(n, _ptr(rowinfo), _ptr(lpack), _ptr(tiles["maxw"]), n_right, _ptr(tile_bound),
-                                     _ptr(mask), stride, _stream()))
+                                     _ptr(perm), _ptr(diag_rank), _ptr(diag_tile_min), _ptr(mask), stride, _stream()))
         _lib.check(L.sg_tiles_candidates(_ptr(perm), n, 0, _ptr(rowinfo), _ptr(lpack), _ptr(mask), stride,
                                          _ptr(tiles["desc"]), _ptr(tiles["blob"]), n_right, B.shape[1],
-                                         _ptr(tile_bound), _ptr(perm_b), tiles["stage_bytes"], _ptr(row_buf),
-                                         _ptr(col_buf), capacity, c_count, c_queue, c_walk, warps, _stream()))
+                                         _ptr(tile_bound), _ptr(perm_b), _ptr(diag_rank), _ptr(diag_tile_min),
+                                         tiles["stage_bytes"], _ptr(row_buf), _ptr(col_buf), capacity, c_count,
+                                         c_queue, c_walk, warps, _stream()))
         LAUNCH_COUNTS["tiles"] += 3
 
     def launch(perm, rb, re_, row_buf, col_buf, capacity, partial_buf=None):
@@ -571,8 +582,8 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
             _ptr(A.d_indptr), _ptr(l_len), _ptr(l_idx), _ptr(l_val), rb, re_, _ptr(perm), n_right,
             A.shape[1], _ptr(bucket_dir), _ptr(bucket_maxw), _ptr(post), _ptr(perm_b), tile_w, acc_code,
             max(B.norm_bound, 1.0),
-            thr_c, _ptr(l_thr), _ptr(l_xp), _ptr(tile_bound), tiles_per_group, _ptr(row_buf), _ptr(col_buf),
-            _ptr(partial_buf), capacity, c_count, c_queue, warps, _stream()))
+            thr_c, _ptr(l_thr), _ptr(l_xp), _ptr(tile_bound), tiles_per_group, _ptr(diag_rank), _ptr(group_items),
+            _ptr(row_buf), _ptr(col_buf), _ptr(partial_buf), capacity, c_count, c_queue, warps, _stream()))
         LAUNCH_COUNTS["candidates"] += 1
 
     # Exact threshold pruning of the left rows (the fixed-point tile always takes per-row thresholds: its margin
@@ -613,7 +624,19 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
     est = None
     first = None          # (cand_row, cand_col, n_cand) of a whole-range launch that needed no sizing pass
     search = True
-    dense = MAX_CAND_DENSITY * n_rows * n_right
+    # (row, column) pairs the launches visit: the triangle holds n (n + 1) / 2 of the n^2
+    dense = MAX_CAND_DENSITY * (n_rows * (n_rows + 1) / 2 if triangle else float(n_rows) * n_right)
+
+    def share(lo, hi):
+        """fraction of the visited pairs that belong to the rows at positions [lo, hi) of the processing order (in the
+        triangle the row at position r visits n - r columns)"""
+        if not triangle:
+            return (hi - lo) / n_rows
+        return ((hi - lo) * n_rows - (lo + hi - 1) * (hi - lo) / 2) / (n_rows * (n_rows + 1) / 2)
+
+    # candidates per chunk: in the triangle every candidate can leave two entries (the pair and its mirror) in the
+    # re-score's output buffers, so a chunk takes half as many to keep its buffers within CAND_CHUNK entries
+    chunk_cand = max(CAND_CHUNK // 2, 1) if triangle else CAND_CHUNK
     # The sizing pass is latency-bound (a few thousand rows against every column tile, cold: 2-3 ms whatever the
     # shard).  While a wasted launch costs no more than a few tens of ms, launch everything at once at the first
     # level into buffers of the density limit; only an overflow or a count above the limit falls back to the
@@ -624,7 +647,7 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
     if not fixed_cap and float(n_rows) * float(n_right) <= OPTIMISTIC_PAIRS:
         prune = levels[0]
         prepare(prune)
-        cap0 = int(min(int(dense) + (1 << 22), CAND_CHUNK))
+        cap0 = int(min(int(dense) + (1 << 22), chunk_cand))
         cand_row0 = _empty(cap0, t.int32, dev)
         cand_col0 = _empty(cap0, t.int32, dev)
         cand_part0 = _empty(cap0, t.float32, dev) if refine else None
@@ -669,19 +692,19 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
             stats["macs_walked"] = int(df[l_idx.long().clamp(0, A.shape[1] - 1)][live].sum().item())
             stats["features_kept"] = int(live.sum().item())
 
-    # Left rows are taken in chunks (slices of the processing order) whose candidates fit CAND_CHUNK entries;
+    # Left rows are taken in chunks (slices of the processing order) whose candidates fit chunk_cand entries;
     # every chunk is re-scored exactly right away and only the pairs strictly above the threshold are kept.
-    n_chunks = 1 if est is None else max(1, -(-int(1.3 * est) // CAND_CHUNK))
+    n_chunks = 1 if est is None else max(1, -(-int(1.3 * est) // chunk_cand))
     rows_per_chunk = -(-n_rows // n_chunks)
     kept = []
-    n_cand_total = 0
+    n_cand_total = n_above = 0
     max_row_cnt = 0
     row_cnt = t.zeros(n_rows + 1, dtype=t.int32, device=dev)      # survivors per left row (sg_rescore)
     for lo in range(0, n_rows, rows_per_chunk):
         hi = min(lo + rows_per_chunk, n_rows)
         perm_chunk = perm_a if (lo == 0 and hi == n_rows) else perm_a[lo:hi]
         if est is not None:
-            cap = min(max(int(1.3 * est * (hi - lo) / n_rows) + (1 << 22), 1 << 22), 1 << 31)
+            cap = min(max(int(1.3 * est * share(lo, hi)) + (1 << 22), 1 << 22), 1 << 31)
         for attempt in range(3):
             if first is not None:
                 cand_row, cand_col, cand_part, n_cand = first
@@ -701,27 +724,30 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
             raise OverflowError("candidate buffer overflow")
         n_cand_total += n_cand
         mark(stats, "candidates")
-        # exact scores; only the candidates strictly above the threshold go on to the selection sorts
-        score = _empty(n_cand, t.float64, dev)
-        keep_row = _empty(n_cand, t.int32, dev)
-        keep_col = _empty(n_cand, t.int32, dev)
+        # exact scores; only the candidates strictly above the threshold go on to the selection sorts (in the
+        # triangle with their mirrored pairs: up to twice as many)
+        n_out = 2 * n_cand if triangle else n_cand
+        score = _empty(n_out, t.float64, dev)
+        keep_row = _empty(n_out, t.int32, dev)
+        keep_col = _empty(n_out, t.int32, dev)
         counters.zero_()
         if refine and cand_part is not None and l_xg is not None:
             _lib.check(L.sg_rescore_refined(n_cand, _ptr(cand_row), _ptr(cand_col), _ptr(cand_part), _ptr(l_xg),
                                             _ptr(B._heavy_groups), _ptr(l_thr), _ptr(A.d_indptr), _ptr(A.d_indices),
                                             _ptr(A.d_val), _ptr(B.d_indptr), _ptr(B.d_indices), _ptr(B.d_val), dt,
                                             _ptr(score), float(threshold), _ptr(keep_row), _ptr(keep_col), c_count,
-                                            c_walk, _ptr(row_cnt), row_begin, _stream()))
+                                            c_walk, c_mirror, _ptr(row_cnt), row_begin, _stream()))
         else:
             _lib.check(L.sg_rescore(n_cand, _ptr(cand_row), _ptr(cand_col), _ptr(A.d_indptr), _ptr(A.d_indices),
                                     _ptr(A.d_val), _ptr(B.d_indptr), _ptr(B.d_indices), _ptr(B.d_val), dt,
                                     _ptr(score), float(threshold), _ptr(keep_row), _ptr(keep_col), c_count,
-                                    _ptr(row_cnt), row_begin, _stream()))
+                                    c_mirror, _ptr(row_cnt), row_begin, _stream()))
         LAUNCH_COUNTS["rescore"] += 1
         if lo + rows_per_chunk >= n_rows:      # last chunk: the largest row rides along with the read-back
             _lib.check(L.sg_row_count_max(n_rows, _ptr(row_cnt), c_queue, _stream()))      # counters[1], zeroed above
-        head = counters[:3].cpu().numpy()
+        head = counters[:4].cpu().numpy()
         n_keep, max_row_cnt = int(head[0]), int(head[1])
+        n_above += n_keep - int(head[3])          # the pairs the re-score kept itself, before mirroring
         if refine and stats is not None:
             stats["n_refined"] = stats.get("n_refined", 0) + int(head[2])
         mark(stats, "rescore")
@@ -739,7 +765,8 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
     del kept
     if stats is not None:
         stats["n_candidates"] = n_cand_total
-        stats["n_above_threshold"] = n_cand
+        stats["n_above_threshold"] = n_above
+        stats["triangle"] = triangle
         stats["n_row_chunks"] = n_chunks
         stats["tile_w"], stats["warps"], stats["n_tiles"] = tile_w, warps, T
         stats["tiles_per_group"] = tiles_per_group

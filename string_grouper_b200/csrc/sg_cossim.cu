@@ -249,6 +249,13 @@ __device__ __forceinline__ void apply_buckets(AccT *__restrict__ acc, const uint
 // are evaluated at once, two tiles per lane in packed fp16 (one HFMA2 per kept feature and tile pair), and only
 // the tiles whose bound can exceed their candidate threshold are walked at all: nothing is accumulated, cleared
 // or swept for the others.
+//
+// Triangle of a self-match (`diag_rank` != NULL, left and right rows the same matrix in the same processing order):
+// row i only reports columns whose position in that order is >= diag_rank[i], so every unordered pair is found
+// once, from the row that comes first (the caller mirrors the kept pairs).  Tiles wholly below the rank are left
+// out of the block-max ballot; in the tile holding the rank the columns below it are not reported.
+// `group_items` (with diag_rank): exclusive offsets of the work items per column-tile group (diag_items_kernel), so
+// that no item is handed out whose row has no tile at or above its rank in the group.
 template <int NW, typename AccT>
 __global__ void __launch_bounds__(NW * 32, min_ctas(NW))
 cossim_candidates_kernel(const int64_t *__restrict__ a_indptr, const int32_t *__restrict__ a_len,
@@ -258,7 +265,8 @@ cossim_candidates_kernel(const int64_t *__restrict__ a_indptr, const int32_t *__
                          const uint32_t *__restrict__ post, const int32_t *__restrict__ perm_b, int Tp, int W,
                          int64_t T, int64_t tiles_per_group, float a_scale, float thr_all,
                          const float *__restrict__ thr_row, const float *__restrict__ xp_norm,
-                         const float *__restrict__ tile_bound, int32_t *__restrict__ cand_row,
+                         const float *__restrict__ tile_bound, const int32_t *__restrict__ diag_rank,
+                         const unsigned long long *__restrict__ group_items, int32_t *__restrict__ cand_row,
                          int32_t *__restrict__ cand_col, float *__restrict__ cand_partial, unsigned long long cap,
                          unsigned long long *__restrict__ cand_count, unsigned long long *__restrict__ row_queue) {
     typedef AccOps<AccT> Ops;
@@ -279,15 +287,23 @@ cossim_candidates_kernel(const int64_t *__restrict__ a_indptr, const int32_t *__
     // large the right matrix is.  tiles_per_group is a multiple of 64.
     const int64_t n_rows = row_end - row_begin;
     const int64_t n_groups = (T + tiles_per_group - 1) / tiles_per_group;
-    const unsigned long long n_items = (unsigned long long)n_rows * (unsigned long long)n_groups;
+    const unsigned long long n_items =
+        group_items ? group_items[n_groups] : (unsigned long long)n_rows * (unsigned long long)n_groups;
     const int n_tiles = (int)T;
+    int64_t group = 0;          // with group_items: items arrive in increasing order, so the group only moves forward
     for (;;) {
         unsigned long long item = 0;
         if (lane == 0) item = atomicAdd(row_queue, 1ull);
         item = __shfl_sync(FULL, item, 0);
         if (item >= n_items) break;
-        const int64_t group = (int64_t)(item / (unsigned long long)n_rows);
-        const int64_t ridx = (int64_t)(item % (unsigned long long)n_rows);
+        int64_t ridx;
+        if (group_items) {
+            while (item >= group_items[group + 1]) ++group;
+            ridx = (int64_t)(item - group_items[group]);
+        } else {
+            group = (int64_t)(item / (unsigned long long)n_rows);
+            ridx = (int64_t)(item % (unsigned long long)n_rows);
+        }
         const int64_t row = perm_a ? perm_a[ridx] : row_begin + ridx;   // processing order: neighbours share buckets
         const int64_t p0 = a_indptr[row];
         const int nf = a_len ? a_len[row] : (int)(a_indptr[row + 1] - p0);
@@ -297,6 +313,10 @@ cossim_candidates_kernel(const int64_t *__restrict__ a_indptr, const int32_t *__
         // tile ids, directory slots (T * V1 < 2^31, checked by sg_postings_build) and positions fit 32 bits
         const int t_begin = (int)(group * tiles_per_group);
         const int t_end = (int)(t_begin + tiles_per_group < T ? t_begin + tiles_per_group : T);
+        // first column position this row reports (0: the full product); tile t holds positions [t*W, t*W + W)
+        const int dr = diag_rank ? diag_rank[row] : 0;
+        const int t_first = (int)(((int64_t)dr / W) & ~63);            // first 64-tile batch at or above the rank
+        const int tb_begin = t_first > t_begin ? t_first : t_begin;
 
         // the first 32 features of the row stay in registers
         int f0 = 0;
@@ -313,9 +333,11 @@ cossim_candidates_kernel(const int64_t *__restrict__ a_indptr, const int32_t *__
         // fp16 arithmetic of the bound: one rounding of at most 2^-11 (values below 2) per kept feature
         const float slack = 5e-4f * (float)nk + 1e-4f;
 
-        for (int tb = t_begin; tb < t_end; tb += 64) {
-            // ---- bounds of tiles tb + 2*lane and tb + 2*lane + 1
+        for (int tb = tb_begin; tb < t_end; tb += 64) {
+            // ---- bounds of tiles tb + 2*lane and tb + 2*lane + 1 (tiles wholly below the rank are not taken)
             unsigned m_even, m_odd;
+            const int t0 = tb + 2 * lane;
+            const bool up0 = (t0 + 1) * W > dr, up1 = (t0 + 2) * W > dr;
             if (nf <= 32) {
                 __half2 ub2 = __float2half2_rn(0.f);
                 const uint32_t *mrow = maxw_h + (tb >> 1) + lane;
@@ -336,15 +358,13 @@ cossim_candidates_kernel(const int64_t *__restrict__ a_indptr, const int32_t *__
                 }
                 const float2 ub = __half22float2(ub2);
                 const float2 tb2 = reinterpret_cast<const float2 *>(tile_bound)[(tb >> 1) + lane];
-                const int t0 = tb + 2 * lane;
                 const float thr0 = xp > 0.f ? fmaxf(fmaf(-xp, tb2.x, thr_r), 0.f) : thr_r;
                 const float thr1 = xp > 0.f ? fmaxf(fmaf(-xp, tb2.y, thr_r), 0.f) : thr_r;
-                m_even = __ballot_sync(FULL, t0 < t_end && ub.x + slack > thr0);
-                m_odd = __ballot_sync(FULL, t0 + 1 < t_end && ub.y + slack > thr1);
+                m_even = __ballot_sync(FULL, t0 < t_end && up0 && ub.x + slack > thr0);
+                m_odd = __ballot_sync(FULL, t0 + 1 < t_end && up1 && ub.y + slack > thr1);
             } else {        // rows with more than 32 kept features: every tile is walked
-                const int t0 = tb + 2 * lane;
-                m_even = __ballot_sync(FULL, t0 < t_end);
-                m_odd = __ballot_sync(FULL, t0 + 1 < t_end);
+                m_even = __ballot_sync(FULL, t0 < t_end && up0);
+                m_odd = __ballot_sync(FULL, t0 + 1 < t_end && up1);
             }
             // ---- walk the surviving tiles; the directory entry of the next one is fetched ahead
             int t = -1;
@@ -391,6 +411,9 @@ cossim_candidates_kernel(const int64_t *__restrict__ a_indptr, const int32_t *__
                             if (v.x | v.y | v.z | v.w) {
                                 acc16[c] = zero4;
                                 m = Ops::above(v, thr_c);
+                                // the tile holding the rank: columns before it belong to earlier rows
+                                const int below = dr - (t * W + c * Ops::PER16);
+                                if (below > 0) m = below >= Ops::PER16 ? 0u : m & (~0u << below);
                             }
                         }
                         if (__any_sync(FULL, m != 0)) {
@@ -424,6 +447,48 @@ cossim_candidates_kernel(const int64_t *__restrict__ a_indptr, const int32_t *__
             }
         }
     }
+}
+
+// Work items of the triangle.  A row has work in the groups from the one holding its rank on, so group g needs the
+// items ridx < last[g] = 1 + the largest ridx whose first group is <= g (a prefix of the launch; exact when the ranks
+// grow with ridx, as for the whole processing order and its slices and strides).
+// Pass 1: last[first group of ridx] = max(ridx + 1), one atomic per warp and group.
+__global__ void diag_last_kernel(int64_t n_rows, const int32_t *__restrict__ perm_a, int64_t row_begin,
+                                 const int32_t *__restrict__ diag_rank, int64_t group_cols,
+                                 unsigned long long *__restrict__ last) {
+    const int64_t ridx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    long long g = -1;
+    if (ridx < n_rows) g = diag_rank[perm_a ? perm_a[ridx] : row_begin + ridx] / group_cols;
+    const unsigned peers = __match_any_sync(FULL, g);
+    if (g >= 0 && lane_id() == 31 - __clz(peers)) atomicMax(last + g, (unsigned long long)(ridx + 1));
+}
+
+// Pass 2 (one warp): running maximum of last[] = items of each group, then their exclusive sum, in place;
+// items[n_groups] = all items.
+__global__ void diag_items_kernel(int64_t n_groups, unsigned long long *__restrict__ items) {
+    const int lane = threadIdx.x;
+    unsigned long long run_max = 0, run_sum = 0;
+    for (int64_t g0 = 0; g0 < n_groups; g0 += 32) {
+        const int64_t g = g0 + lane;
+        unsigned long long v = g < n_groups ? items[g] : 0ull;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const unsigned long long up = __shfl_up_sync(FULL, v, o);
+            if (lane >= o && up > v) v = up;
+        }
+        if (run_max > v) v = run_max;
+        run_max = __shfl_sync(FULL, v, 31);
+        if (g >= n_groups) v = 0;                       // lanes past the last group add nothing
+        unsigned long long s = v;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const unsigned long long up = __shfl_up_sync(FULL, s, o);
+            if (lane >= o) s += up;
+        }
+        if (g < n_groups) items[g] = run_sum + s - v;
+        run_sum += __shfl_sync(FULL, s, 31);
+    }
+    if (lane == 0) items[n_groups] = run_sum;
 }
 
 // ---------------------------------------------------------------------------
@@ -508,6 +573,44 @@ __device__ __forceinline__ T merge_dot_vec(const int32_t *__restrict__ ai, const
 // exceeds `keep_thr` (strict, string_grouper.py:729/:740) survive, appended in no particular order to
 // (keep_row, keep_col, out) through one warp-aggregated atomic per warp: the selection sorts that follow then
 // work on the matches-to-be instead of on every candidate the pruned traversal had to report.
+//
+// Mirror (`mirror_count` != NULL, the triangle of a self-match): every kept pair (r, c) with r != c is also written
+// as (c, r) with the same score, right behind the warp's own pairs.  The mirrored score is the exact one: the
+// sorted merge multiplies the same two values in the other order (IEEE products commute) and adds the products in
+// the same ascending feature order, so score(c, r) is score(r, c) bit for bit.
+__device__ __forceinline__ void keep_pairs(bool keep, bool mir, int32_t r, int32_t c, double sc, int lane,
+                                           int32_t *__restrict__ keep_row, int32_t *__restrict__ keep_col,
+                                           double *__restrict__ out, unsigned long long *__restrict__ keep_count,
+                                           unsigned long long *__restrict__ mirror_count,
+                                           int32_t *__restrict__ row_cnt, int64_t row_begin) {
+    const unsigned m = __ballot_sync(FULL, keep);
+    if (!m) return;
+    const unsigned mm = __ballot_sync(FULL, mir);
+    const int leader = __ffs(m) - 1;
+    unsigned long long base = 0;
+    if (lane == leader) {
+        base = atomicAdd(keep_count, (unsigned long long)(__popc(m) + __popc(mm)));
+        if (mm) atomicAdd(mirror_count, (unsigned long long)__popc(mm));
+    }
+    base = __shfl_sync(FULL, base, leader);
+    const unsigned lt = (1u << lane) - 1u;
+    if (keep) {
+        const unsigned long long w = base + __popc(m & lt);
+        keep_row[w] = r;
+        keep_col[w] = c;
+        out[w] = sc;
+        if (row_cnt) atomicAdd(row_cnt + (r - row_begin), 1);       // survivors per row: sizes the row buckets of
+                                                                    // sg_topn_select_rows
+    }
+    if (mir) {
+        const unsigned long long w = base + __popc(m) + __popc(mm & lt);
+        keep_row[w] = c;
+        keep_col[w] = r;
+        out[w] = sc;
+        if (row_cnt) atomicAdd(row_cnt + (c - row_begin), 1);
+    }
+}
+
 template <typename T, int VEC>
 __global__ void __launch_bounds__(256, 8) rescore_kernel(int64_t n, const int32_t *__restrict__ cr, const int32_t *__restrict__ cc,
                                const int64_t *__restrict__ a_indptr, const int32_t *__restrict__ a_idx,
@@ -515,7 +618,8 @@ __global__ void __launch_bounds__(256, 8) rescore_kernel(int64_t n, const int32_
                                const int32_t *__restrict__ b_idx, const T *__restrict__ b_val,
                                double *__restrict__ out, double keep_thr, int32_t *__restrict__ keep_row,
                                int32_t *__restrict__ keep_col, unsigned long long *__restrict__ keep_count,
-                               int32_t *__restrict__ row_cnt, int64_t row_begin) {
+                               unsigned long long *__restrict__ mirror_count, int32_t *__restrict__ row_cnt,
+                               int64_t row_begin) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     int32_t r = 0, c = 0;
     double sc = 0.0;
@@ -531,20 +635,8 @@ __global__ void __launch_bounds__(256, 8) rescore_kernel(int64_t n, const int32_
         keep = keep_count && sc > keep_thr;
     }
     if (!keep_count) return;
-    const unsigned m = __ballot_sync(FULL, keep);
-    if (!m) return;
-    const int lane = threadIdx.x & 31;
-    unsigned long long base = 0;
-    if (lane == __ffs(m) - 1) base = atomicAdd(keep_count, (unsigned long long)__popc(m));
-    base = __shfl_sync(FULL, base, __ffs(m) - 1);
-    if (keep) {
-        const unsigned long long w = base + __popc(m & ((1u << lane) - 1u));
-        keep_row[w] = r;
-        keep_col[w] = c;
-        out[w] = sc;
-        if (row_cnt) atomicAdd(row_cnt + (r - row_begin), 1);       // survivors per row: sizes the row buckets of
-                                                                    // sg_topn_select_rows
-    }
+    keep_pairs(keep, keep && mirror_count && r != c, r, c, sc, threadIdx.x & 31, keep_row, keep_col, out, keep_count,
+               mirror_count, row_cnt, row_begin);
 }
 
 // sg_rescore_refined: a CTA takes REFINE_CHUNK consecutive candidates.  Pass 1 re-tests each with the grouped bound
@@ -579,7 +671,8 @@ rescore_refined_kernel(int64_t n, const int32_t *__restrict__ cr, const int32_t 
                        const int32_t *__restrict__ b_idx, const T *__restrict__ b_val, double *__restrict__ out,
                        double keep_thr, int32_t *__restrict__ keep_row, int32_t *__restrict__ keep_col,
                        unsigned long long *__restrict__ keep_count, unsigned long long *__restrict__ refined_count,
-                       int32_t *__restrict__ row_cnt, int64_t row_begin) {
+                       unsigned long long *__restrict__ mirror_count, int32_t *__restrict__ row_cnt,
+                       int64_t row_begin) {
     __shared__ uint16_t live[REFINE_CHUNK];
     __shared__ int n_live;
     const int lane = threadIdx.x & 31;
@@ -619,18 +712,8 @@ rescore_refined_kernel(int64_t n, const int32_t *__restrict__ cr, const int32_t 
                                             b_indptr[c + 1]);
             keep = sc > keep_thr;
         }
-        const unsigned m = __ballot_sync(FULL, keep);
-        if (!m) continue;
-        unsigned long long w0 = 0;
-        if (lane == __ffs(m) - 1) w0 = atomicAdd(keep_count, (unsigned long long)__popc(m));
-        w0 = __shfl_sync(FULL, w0, __ffs(m) - 1);
-        if (keep) {
-            const unsigned long long w = w0 + __popc(m & ((1u << lane) - 1u));
-            keep_row[w] = r;
-            keep_col[w] = c;
-            out[w] = sc;
-            if (row_cnt) atomicAdd(row_cnt + (r - row_begin), 1);
-        }
+        keep_pairs(keep, keep && mirror_count && r != c, r, c, sc, lane, keep_row, keep_col, out, keep_count,
+                   mirror_count, row_cnt, row_begin);
     }
 }
 
@@ -822,6 +905,7 @@ static int launch_candidates(const int64_t *a_indptr, const int32_t *a_len, cons
                              const void *postings, const int32_t *perm_b, int tile_w, int64_t tiles_per_group,
                              float a_scale,
                              float thr_c, const float *thr_row, const float *xp_norm, const float *tile_bound,
+                             const int32_t *diag_rank, unsigned long long *group_items,
                              int32_t *cand_row, int32_t *cand_col, float *cand_partial,
                              int64_t cand_cap, unsigned long long *cand_count, unsigned long long *row_queue,
                              int n_sm, cudaStream_t st) {
@@ -830,6 +914,15 @@ static int launch_candidates(const int64_t *a_indptr, const int32_t *a_len, cons
                                      (int)smem));
     const int64_t T = sg_num_tiles(n_right, tile_w);
     const int64_t n_rows = row_end - row_begin;
+    if (diag_rank) {
+        const int64_t n_groups = (T + tiles_per_group - 1) / tiles_per_group;
+        SG_CUDA_TRY(cudaMemsetAsync(group_items, 0, (size_t)(n_groups + 1) * sizeof(unsigned long long), st));
+        diag_last_kernel<<<(unsigned)((n_rows + 255) / 256), 256, 0, st>>>(n_rows, perm_a, row_begin, diag_rank,
+                                                                           tiles_per_group * tile_w, group_items);
+        SG_LAUNCH_CHECK();
+        diag_items_kernel<<<1, 32, 0, st>>>(n_groups, group_items);
+        SG_LAUNCH_CHECK();
+    }
     int per_sm = 1;
     SG_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, cossim_candidates_kernel<NW, AccT>, NW * 32,
                                                               smem));
@@ -841,8 +934,8 @@ static int launch_candidates(const int64_t *a_indptr, const int32_t *a_len, cons
         a_indptr, a_len, a_indices, a_val32, row_begin, row_end, perm_a, n_right, (const int2 *)bucket_dir,
         (const uint32_t *)bucket_maxw, (const uint32_t *)postings, perm_b, (int)sg_num_tiles_padded(n_right, tile_w),
         tile_w, T, tiles_per_group,
-        a_scale, thr_c, thr_row, xp_norm, tile_bound, cand_row, cand_col, cand_partial, (unsigned long long)cand_cap,
-        cand_count, row_queue);
+        a_scale, thr_c, thr_row, xp_norm, tile_bound, diag_rank, diag_rank ? group_items : nullptr, cand_row, cand_col,
+        cand_partial, (unsigned long long)cand_cap, cand_count, row_queue);
     SG_LAUNCH_CHECK();
     return SG_OK;
 }
@@ -855,14 +948,16 @@ int sg_cossim_candidates(const int64_t *a_indptr, const int32_t *a_len, const in
                          const void *postings, const int32_t *perm_b, int tile_w, int acc_dtype, float a_scale,
                          float cand_threshold,
                          const float *cand_threshold_row, const float *pruned_norm_row, const float *tile_bound,
-                         int64_t tiles_per_group, int32_t *cand_row,
-                         int32_t *cand_col, float *cand_partial, int64_t cand_cap, unsigned long long *cand_count,
-                         unsigned long long *row_queue, int warps_per_cta, void *stream_) {
+                         int64_t tiles_per_group, const int32_t *diag_rank, unsigned long long *group_items,
+                         int32_t *cand_row, int32_t *cand_col, float *cand_partial, int64_t cand_cap,
+                         unsigned long long *cand_count, unsigned long long *row_queue, int warps_per_cta,
+                         void *stream_) {
     cudaStream_t st = (cudaStream_t)stream_;
     if (row_end <= row_begin || n_right <= 0) return SG_OK;
     if (acc_dtype != SG_ACC_F32 && acc_dtype != SG_ACC_U16)
         return fail(SG_ERR_INVALID, "acc_dtype must be SG_ACC_F32 or SG_ACC_U16");
     if (!tile_bound || !bucket_maxw) return fail(SG_ERR_INVALID, "tile_bound and bucket_maxw are required");
+    if (diag_rank && !group_items) return fail(SG_ERR_INVALID, "diag_rank needs group_items");
     if (tiles_per_group < 64 || tiles_per_group % 64)
         return fail(SG_ERR_INVALID, "tiles_per_group must be a positive multiple of 64");
     const int acc_bytes = acc_dtype == SG_ACC_U16 ? 2 : 4;
@@ -880,7 +975,7 @@ int sg_cossim_candidates(const int64_t *a_indptr, const int32_t *a_len, const in
 #define SG_ARGS                                                                                              \
     a_indptr, a_len, a_indices, a_val32, row_begin, row_end, perm_a, n_right, n_cols, bucket_dir, bucket_maxw, \
         postings, perm_b, tile_w, tiles_per_group, a_scale, cand_threshold, cand_threshold_row, pruned_norm_row,      \
-        tile_bound, cand_row, cand_col, cand_partial, cand_cap, cand_count, row_queue, n_sm, st
+        tile_bound, diag_rank, group_items, cand_row, cand_col, cand_partial, cand_cap, cand_count, row_queue, n_sm, st
 #define SG_CASE(NW)                                                                                          \
     case NW:                                                                                                 \
         return acc_dtype == SG_ACC_U16 ? launch_candidates<NW, uint16_t>(SG_ARGS)                           \
@@ -900,18 +995,19 @@ int sg_cossim_candidates(const int64_t *a_indptr, const int32_t *a_len, const in
 int sg_rescore(int64_t n_cand, const int32_t *cand_row, const int32_t *cand_col, const int64_t *a_indptr,
                const int32_t *a_indices, const void *a_val, const int64_t *b_indptr, const int32_t *b_indices,
                const void *b_val, int dtype, double *score_out, double keep_threshold, int32_t *keep_row,
-               int32_t *keep_col, unsigned long long *keep_count, int32_t *row_cnt, int64_t row_begin,
-               void *stream_) {
+               int32_t *keep_col, unsigned long long *keep_count, unsigned long long *mirror_count,
+               int32_t *row_cnt, int64_t row_begin, void *stream_) {
     cudaStream_t st = (cudaStream_t)stream_;
     if (n_cand <= 0) return SG_OK;
     if (keep_count && (!keep_row || !keep_col)) return fail(SG_ERR_INVALID, "keep_count needs keep_row and keep_col");
     if (row_cnt && !keep_count) return fail(SG_ERR_INVALID, "row_cnt needs keep_count");
+    if (mirror_count && !keep_count) return fail(SG_ERR_INVALID, "mirror_count needs keep_count");
     const unsigned grid = (unsigned)((n_cand + 255) / 256);
     const bool vec = ((uintptr_t)b_indices & 15) == 0;      // merge_dot_vec reads aligned 16-byte index vectors
 #define SG_RESCORE(T, VEC)                                                                                        \
     rescore_kernel<T, VEC><<<grid, 256, 0, st>>>(n_cand, cand_row, cand_col, a_indptr, a_indices, (const T *)a_val, \
                                                  b_indptr, b_indices, (const T *)b_val, score_out, keep_threshold,  \
-                                                 keep_row, keep_col, keep_count, row_cnt, row_begin)
+                                                 keep_row, keep_col, keep_count, mirror_count, row_cnt, row_begin)
     if (dtype == SG_DTYPE_F64) {
         if (vec) SG_RESCORE(double, 1);
         else SG_RESCORE(double, 0);
@@ -931,8 +1027,8 @@ int sg_rescore_refined(int64_t n_cand, const int32_t *cand_row, const int32_t *c
                        const int64_t *a_indptr, const int32_t *a_indices, const void *a_val,
                        const int64_t *b_indptr, const int32_t *b_indices, const void *b_val, int dtype,
                        double *score_out, double keep_threshold, int32_t *keep_row, int32_t *keep_col,
-                       unsigned long long *keep_count, unsigned long long *refined_count, int32_t *row_cnt,
-                       int64_t row_begin, void *stream_) {
+                       unsigned long long *keep_count, unsigned long long *refined_count,
+                       unsigned long long *mirror_count, int32_t *row_cnt, int64_t row_begin, void *stream_) {
     cudaStream_t st = (cudaStream_t)stream_;
     if (n_cand <= 0) return SG_OK;
     if (!keep_count || !keep_row || !keep_col) return fail(SG_ERR_INVALID, "keep_count, keep_row and keep_col are required");
@@ -946,7 +1042,7 @@ int sg_rescore_refined(int64_t n_cand, const int32_t *cand_row, const int32_t *c
     rescore_refined_kernel<T, VEC><<<grid, 256, 0, st>>>(                                                           \
         n_cand, cand_row, cand_col, cand_partial, (const uint4 *)left_group_norms, (const uint4 *)right_group_norms, \
         row_threshold, a_indptr, a_indices, (const T *)a_val, b_indptr, b_indices, (const T *)b_val, score_out,      \
-        keep_threshold, keep_row, keep_col, keep_count, refined_count, row_cnt, row_begin)
+        keep_threshold, keep_row, keep_col, keep_count, refined_count, mirror_count, row_cnt, row_begin)
     if (dtype == SG_DTYPE_F64) {
         if (vec) SG_RESCORE(double, 1);
         else SG_RESCORE(double, 0);

@@ -257,15 +257,25 @@ constexpr int FL_WARPS = 8;
 constexpr int FL_RANKS = 32;      // ranks per CTA (4 per warp)
 constexpr int FL_WORDS = 128;     // mask words per pass through shared memory (4096 tiles)
 
+// Triangle of a self-match (diag_rank != NULL): tiles wholly below the tile holding the row's own position in the
+// processing order (diag_rank[perm[rank]]) get no bit, and diag_tile_min[CTA] receives the smallest such tile of the
+// CTA's FL_RANKS ranks (sg_tiles_candidates skips the (tile, segment) items below all of their rows).
 __global__ void __launch_bounds__(FL_WARPS * 32)
 tile_filter_kernel(int64_t n_ranks, const int4 *__restrict__ rowinfo, const int2 *__restrict__ lpack,
                    const uint32_t *__restrict__ maxw_h, int Tp, int64_t T, const float *__restrict__ tile_bound,
-                   uint32_t *__restrict__ mask, int64_t mask_stride) {
+                   const int32_t *__restrict__ perm, const int32_t *__restrict__ diag_rank,
+                   uint32_t *__restrict__ diag_tile_min, uint32_t *__restrict__ mask, int64_t mask_stride) {
     __shared__ uint32_t buf[FL_WORDS][FL_RANKS + 1];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int64_t rank0 = (int64_t)blockIdx.x * FL_RANKS;
     const int n_words = Tp >> 5;
     const int half_tp = Tp >> 1;
+    if (diag_rank && warp == 0) {
+        const int64_t r = rank0 + lane;
+        const unsigned dt = r < n_ranks ? (unsigned)(diag_rank[perm[r]] / TL_W) : 0xffffffffu;
+        const unsigned lo = __reduce_min_sync(FULL, dt);
+        if (lane == 0) diag_tile_min[blockIdx.x] = lo;
+    }
     for (int w0 = 0; w0 < n_words; w0 += FL_WORDS) {
         const int w1 = w0 + FL_WORDS < n_words ? w0 + FL_WORDS : n_words;
         for (int ri = 0; ri < FL_RANKS / FL_WARPS; ++ri) {
@@ -273,9 +283,10 @@ tile_filter_kernel(int64_t n_ranks, const int4 *__restrict__ rowinfo, const int2
             const int64_t r = rank0 + rr;
             int nf = 0;
             float thr_r = 0.f, xp = 0.f;
-            int f0 = 0;
+            int f0 = 0, t_diag = 0;
             __half2 a2 = __float2half2_rn(0.f);
             if (r < n_ranks) {
+                if (diag_rank) t_diag = diag_rank[perm[r]] / TL_W;
                 const int4 info = rowinfo[r];
                 nf = info.y;
                 thr_r = __int_as_float(info.z);
@@ -293,9 +304,10 @@ tile_filter_kernel(int64_t n_ranks, const int4 *__restrict__ rowinfo, const int2
                 const int tb = wd << 5;                       // first tile of the batch
                 unsigned m_even = 0, m_odd = 0;
                 const int t0 = tb + 2 * lane;
+                const bool in0 = t0 < T && t0 >= t_diag, in1 = t0 + 1 < T && t0 + 1 >= t_diag;
                 if (nf > 32) {                                // more kept features than lanes: every tile is walked
-                    m_even = __ballot_sync(FULL, t0 < T);
-                    m_odd = __ballot_sync(FULL, t0 + 1 < T);
+                    m_even = __ballot_sync(FULL, in0);
+                    m_odd = __ballot_sync(FULL, in1);
                 } else if (nf > 0) {
                     __half2 ub2 = __float2half2_rn(0.f);
                     const uint32_t *mrow = maxw_h + (tb >> 1) + lane;
@@ -309,8 +321,8 @@ tile_filter_kernel(int64_t n_ranks, const int4 *__restrict__ rowinfo, const int2
                     const float2 tb2 = reinterpret_cast<const float2 *>(tile_bound)[(tb >> 1) + lane];
                     const float thr0 = xp > 0.f ? fmaxf(fmaf(-xp, tb2.x, thr_r), 0.f) : thr_r;
                     const float thr1 = xp > 0.f ? fmaxf(fmaf(-xp, tb2.y, thr_r), 0.f) : thr_r;
-                    m_even = __ballot_sync(FULL, t0 < T && ub.x + slack > thr0);
-                    m_odd = __ballot_sync(FULL, t0 + 1 < T && ub.y + slack > thr1);
+                    m_even = __ballot_sync(FULL, in0 && ub.x + slack > thr0);
+                    m_odd = __ballot_sync(FULL, in1 && ub.y + slack > thr1);
                 }
                 if (lane == 0) {
                     buf[wd - w0][rr] = m_even;
@@ -338,24 +350,35 @@ struct WarpCtx {
     int ccount;
 };
 
+// With diag_rank (the triangle of a self-match) a column before the row's own position in the processing order is
+// not reported: it only occurs in the tile holding that position, and the earlier row reports the pair.
 __device__ __forceinline__ void flush_candidates(WarpCtx &cx, int lane, const int32_t *__restrict__ perm_a,
                                                  int64_t row_begin, const int32_t *__restrict__ perm_b,
+                                                 const int32_t *__restrict__ diag_rank,
                                                  int32_t *__restrict__ cand_row, int32_t *__restrict__ cand_col,
                                                  unsigned long long cap, unsigned long long *cand_count) {
     __syncwarp();
-    if (cx.ccount > 0) {
-        unsigned long long base = 0;
-        if (lane == 0) base = atomicAdd(cand_count, (unsigned long long)cx.ccount);
-        base = __shfl_sync(FULL, base, 0);
-        for (int i = lane; i < cx.ccount; i += 32) {
-            const int2 c = cx.cbuf[i];
-            if (base + i < cap) {
-                cand_row[base + i] = (int32_t)(perm_a ? perm_a[c.x] : row_begin + c.x);
-                cand_col[base + i] = perm_b ? perm_b[c.y] : c.y;
-            }
+    for (int i0 = 0; i0 < cx.ccount; i0 += 32) {
+        const int i = i0 + lane;
+        int2 c = make_int2(0, 0);
+        int32_t row = 0;
+        bool ok = i < cx.ccount;
+        if (ok) {
+            c = cx.cbuf[i];
+            row = (int32_t)(perm_a ? perm_a[c.x] : row_begin + c.x);
+            if (diag_rank) ok = c.y >= diag_rank[row];
         }
-        cx.ccount = 0;
+        const unsigned m = __ballot_sync(FULL, ok);
+        if (!m) continue;
+        unsigned long long base = 0;
+        if (lane == 0) base = atomicAdd(cand_count, (unsigned long long)__popc(m));
+        base = __shfl_sync(FULL, base, 0) + __popc(m & ((1u << lane) - 1u));
+        if (ok && base < cap) {
+            cand_row[base] = row;
+            cand_col[base] = perm_b ? perm_b[c.y] : c.y;
+        }
     }
+    cx.ccount = 0;
     __syncwarp();
 }
 
@@ -367,7 +390,7 @@ __device__ __forceinline__ void flush_candidates(WarpCtx &cx, int lane, const in
             if ((crossed_)) cx.cbuf[cx.ccount + __popc(em_ & lt_mask)] = make_int2(rank_id, col0 + ((int)(colbyte_) >> 2)); \
             cx.ccount += __popc(em_);                                                                     \
             if (cx.ccount > TL_CBUF - 32)                                                                 \
-                flush_candidates(cx, lane, perm_a, row_begin, perm_b, cand_row, cand_col, cap, cand_count);   \
+                flush_candidates(cx, lane, perm_a, row_begin, perm_b, diag_rank, cand_row, cand_col, cap, cand_count);   \
         }                                                                                                 \
     } while (0)
 
@@ -481,6 +504,7 @@ tile_candidates_kernel(const int32_t *__restrict__ perm_a, int64_t n_ranks, int6
                        const uint32_t *__restrict__ mask, int64_t mask_stride, const TileDesc *__restrict__ tdesc,
                        const unsigned char *__restrict__ blob, int64_t T, int bw,
                        const float *__restrict__ tile_bound, const int32_t *__restrict__ perm_b,
+                       const int32_t *__restrict__ diag_rank, const uint32_t *__restrict__ seg_tile_min,
                        int64_t seg_ranks, int64_t n_seg, int32_t *__restrict__ cand_row,
                        int32_t *__restrict__ cand_col, unsigned long long cap,
                        unsigned long long *__restrict__ cand_count, unsigned long long *__restrict__ queue,
@@ -514,7 +538,11 @@ tile_candidates_kernel(const int32_t *__restrict__ perm_a, int64_t n_ranks, int6
     for (;;) {
         // ---- next (tile, rank segment); its blob goes into shared memory by bulk copies (TMA)
         if (threadIdx.x == 0) {
-            const unsigned long long it = atomicAdd(queue, 1ull);
+            unsigned long long it = atomicAdd(queue, 1ull);
+            // triangle: an item whose tile lies below the tile of every row of its segment has no pair
+            while (seg_tile_min && it < n_items &&
+                   it / (unsigned long long)n_seg < seg_tile_min[(it % (unsigned long long)n_seg) * (seg_ranks / FL_RANKS)])
+                it = atomicAdd(queue, 1ull);
             *s_item = (long long)it;
             if (it < n_items) {
                 const TileDesc d = tdesc[it / (unsigned long long)n_seg];
@@ -612,11 +640,23 @@ tile_candidates_kernel(const int32_t *__restrict__ perm_a, int64_t n_ranks, int6
         parity ^= 1u;
         __syncthreads();      // every warp is done with the staged tile before the next one is copied over it
     }
-    flush_candidates(cx, lane, perm_a, row_begin, perm_b, cand_row, cand_col, cap, cand_count);
+    flush_candidates(cx, lane, perm_a, row_begin, perm_b, diag_rank, cand_row, cand_col, cap, cand_count);
     if (walk_stats && lane == 0) {
         atomicAdd(walk_stats, n_pairs);
         atomicAdd(walk_stats + 1, n_walked);
     }
+}
+
+// Smallest diagonal tile of every rank segment, in place: entry s * k of the per-CTA minima of tile_filter_kernel
+// (k = seg_ranks / FL_RANKS CTAs per segment) becomes the minimum over the segment's entries [s * k, s * k + k).
+__global__ void seg_tile_min_kernel(int64_t n_blocks, int64_t k, int64_t n_seg, uint32_t *__restrict__ m) {
+    const int64_t s = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (s >= n_seg) return;
+    const int64_t e = (s + 1) * k < n_blocks ? (s + 1) * k : n_blocks;
+    unsigned lo = 0xffffffffu;
+    for (int64_t i = s * k + lane_id(); i < e; i += 32) lo = min(lo, m[i]);
+    lo = __reduce_min_sync(FULL, lo);
+    if (lane_id() == 0) m[s * k] = lo;
 }
 
 static int bits_for64(uint64_t v) {
@@ -732,15 +772,17 @@ int64_t sg_tiles_mask_words(int64_t n_right) { return sg_num_tiles_padded(n_righ
 
 /* survivors of the block-max test: mask[word * mask_stride + rank], mask_stride = n_ranks rounded up to 32 */
 int sg_tiles_filter(int64_t n_ranks, const void *rowinfo, const void *lpack, const void *bucket_maxw,
-                    int64_t n_right, const float *tile_bound, uint32_t *mask, int64_t mask_stride, void *stream_) {
+                    int64_t n_right, const float *tile_bound, const int32_t *perm, const int32_t *diag_rank,
+                    uint32_t *diag_tile_min, uint32_t *mask, int64_t mask_stride, void *stream_) {
     cudaStream_t st = (cudaStream_t)stream_;
     if (n_ranks <= 0 || n_right <= 0) return SG_OK;
     if (mask_stride < n_ranks || (mask_stride & 31)) return fail(SG_ERR_INVALID, "mask_stride must be n_ranks rounded up to 32");
+    if (diag_rank && (!perm || !diag_tile_min)) return fail(SG_ERR_INVALID, "diag_rank needs perm and diag_tile_min");
     const int64_t T = sg_num_tiles(n_right, TL_W);
     const int Tp = (int)sg_num_tiles_padded(n_right, TL_W);
     tile_filter_kernel<<<(unsigned)(mask_stride / FL_RANKS), FL_WARPS * 32, 0, st>>>(
-        n_ranks, (const int4 *)rowinfo, (const int2 *)lpack, (const uint32_t *)bucket_maxw, Tp, T, tile_bound, mask,
-        mask_stride);
+        n_ranks, (const int4 *)rowinfo, (const int2 *)lpack, (const uint32_t *)bucket_maxw, Tp, T, tile_bound, perm,
+        diag_rank, diag_tile_min, mask, mask_stride);
     SG_LAUNCH_CHECK();
     return SG_OK;
 }
@@ -752,12 +794,13 @@ size_t sg_tiles_smem_bytes(int stage_bytes, int warps_per_cta) {
 int sg_tiles_candidates(const int32_t *perm_a, int64_t n_ranks, int64_t row_begin, const void *rowinfo,
                         const void *lpack, const uint32_t *mask, int64_t mask_stride, const void *tile_desc,
                         const void *blob, int64_t n_right, int64_t n_cols, const float *tile_bound,
-                        const int32_t *perm_b, int stage_bytes, int32_t *cand_row, int32_t *cand_col,
-                        int64_t cand_cap, unsigned long long *cand_count, unsigned long long *queue,
-                        unsigned long long *walk_stats, int warps_per_cta, void *stream_) {
+                        const int32_t *perm_b, const int32_t *diag_rank, uint32_t *diag_tile_min, int stage_bytes,
+                        int32_t *cand_row, int32_t *cand_col, int64_t cand_cap, unsigned long long *cand_count,
+                        unsigned long long *queue, unsigned long long *walk_stats, int warps_per_cta, void *stream_) {
     cudaStream_t st = (cudaStream_t)stream_;
     if (n_ranks <= 0 || n_right <= 0) return SG_OK;
     if (warps_per_cta != 8 && warps_per_cta != 16) return fail(SG_ERR_INVALID, "warps_per_cta must be 8 or 16");
+    if (diag_rank && (!perm_a || !diag_tile_min)) return fail(SG_ERR_INVALID, "diag_rank needs perm_a and diag_tile_min");
     int dev = 0, n_sm = 0, smem_optin = 0;
     SG_CUDA_TRY(cudaGetDevice(&dev));
     SG_CUDA_TRY(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
@@ -785,10 +828,17 @@ int sg_tiles_candidates(const int32_t *perm_a, int64_t n_ranks, int64_t row_begi
         seg_ranks = ((n_ranks + n_seg - 1) / n_seg + 255) / 256 * 256;                                               \
         n_seg = (n_ranks + seg_ranks - 1) / seg_ranks;                                                               \
         if (ctas > T * n_seg) ctas = T * n_seg;                                                                      \
+        if (diag_rank) {                                                                                             \
+            seg_tile_min_kernel<<<(unsigned)((n_seg + 7) / 8), 256, 0, st>>>(mask_stride / FL_RANKS,                 \
+                                                                            seg_ranks / FL_RANKS, n_seg,             \
+                                                                            diag_tile_min);                          \
+            SG_LAUNCH_CHECK();                                                                                       \
+        }                                                                                                            \
         tile_candidates_kernel<NW><<<(unsigned)ctas, NW * 32, smem, st>>>(                                           \
             perm_a, n_ranks, row_begin, (const int4 *)rowinfo, (const int2 *)lpack, mask, mask_stride,               \
-            (const TileDesc *)tile_desc, (const unsigned char *)blob, T, bw, tile_bound, perm_b, seg_ranks, n_seg,   \
-            cand_row, cand_col, (unsigned long long)cand_cap, cand_count, queue, walk_stats, stage_bytes);           \
+            (const TileDesc *)tile_desc, (const unsigned char *)blob, T, bw, tile_bound, perm_b, diag_rank,          \
+            diag_rank ? diag_tile_min : nullptr, seg_ranks, n_seg, cand_row, cand_col, (unsigned long long)cand_cap, \
+            cand_count, queue, walk_stats, stage_bytes);                                                             \
     } while (0)
     if (warps_per_cta == 16) SG_TL_LAUNCH(16); else SG_TL_LAUNCH(8);
 #undef SG_TL_LAUNCH
