@@ -194,6 +194,17 @@ int sg_prune_rows(int64_t row_begin, int64_t row_end, const int64_t *indptr /*[d
                                           heavy ranks (csrc/sg_prune.cu: ranks 0..13 alone, 14..38, 39..63), rounded
                                           up; needs `prunable` = sg_heavy_features ranks*/,
                   void *stream);
+/* sg_prune_rows with a per-row threshold: row i is pruned for t_i = max(threshold, row_floor[i] - 1e-6) (the
+ * pairs that can still reach a top-n floor, sg_cossim_candidates_floor) with budget frac * (t_i - margin), and
+ * out_threshold[i] = t_i - margin - margin_per_feature * kept. */
+int sg_prune_rows_floor(int64_t row_begin, int64_t row_end, const int64_t *indptr /*[dev]*/,
+                        const int32_t *indices /*[dev]*/, const float *val32 /*[dev]*/,
+                        const int32_t *df_right /*[dev] n_cols*/, const int8_t *prunable /*[dev] n_cols or NULL*/,
+                        float right_norm, float frac /* in [0, 1) */, float threshold,
+                        const float *row_floor /*[dev] per row id*/, float margin, float margin_per_feature,
+                        int32_t *out_indices /*[dev]*/, float *out_val32 /*[dev]*/, int32_t *out_len /*[dev]*/,
+                        float *out_threshold /*[dev]*/, float *out_pruned_norm /*[dev]*/,
+                        void *out_group_norms /*[dev] or NULL*/, void *stream);
 int sg_heavy_norms(int64_t row_begin, int64_t row_end, const int64_t *indptr /*[dev]*/,
                    const int32_t *indices /*[dev]*/, const float *val32 /*[dev]*/, const int8_t *hrank /*[dev]*/,
                    float *out_norm /*[dev] row_end-row_begin*/,
@@ -246,6 +257,34 @@ int sg_cossim_candidates(const int64_t *a_indptr /*[dev]*/, const int32_t *a_len
                          int64_t cand_cap,
                          unsigned long long *cand_count /*[dev] 1*/,
                          unsigned long long *row_queue /*[dev] 1*/, int warps_per_cta, void *stream);
+/*
+ * sg_cossim_candidates with a top-n floor (1 <= top_n <= 32, non-negative weights, warps_per_cta = 8, no triangle).
+ * `row_floor` [dev, per left row id, float, zeroed before the first launch of a product] holds a proven lower bound
+ * of the exact score of each row's top_n-th best pair and only rises.  A pair is reported when its partial score
+ * exceeds max(threshold of the row, row_floor[row] - 1e-6 - E_r) - pruned_norm_row[row] * tile_bound[tile], with
+ * E_r = floor_margin + floor_margin_per_feature * (kept features): the same margins the caller subtracted from the
+ * row thresholds, which also bound how far a partial score can EXCEED the kept-feature product.  Every work item
+ * keeps the best 32 values (partial - E_r, rounded down) of the pairs it reported and, once it holds top_n of them,
+ * raises row_floor[row] to the top_n-th with atomicMax; the floor is read again at every batch of 64 column tiles.
+ * Self-match (`self_rank` [dev] per row id: the row's position in the common processing order, perm_a the same
+ * order): `seed` = 1 walks only the column-tile group holding the row, starting at the 64-tile batch that holds it;
+ * seed = 0 walks every other group.  self_rank = NULL: every group (two matrices).
+ */
+int sg_cossim_candidates_floor(const int64_t *a_indptr /*[dev]*/, const int32_t *a_len /*[dev] or NULL*/,
+                               const int32_t *a_indices /*[dev]*/, const float *a_val32 /*[dev]*/,
+                               int64_t row_begin, int64_t row_end, const int32_t *perm_a /*[dev] or NULL*/,
+                               int64_t n_right, int64_t n_cols, const void *bucket_dir /*[dev]*/,
+                               const void *bucket_maxw /*[dev]*/, const void *postings /*[dev]*/,
+                               const int32_t *perm_b /*[dev] or NULL*/, int tile_w, int acc_dtype, float a_scale,
+                               float cand_threshold, const float *cand_threshold_row /*[dev] per row id, or NULL*/,
+                               const float *pruned_norm_row /*[dev] per row id, or NULL*/,
+                               const float *tile_bound /*[dev]*/, int64_t tiles_per_group,
+                               int32_t *cand_row /*[dev] cap*/, int32_t *cand_col /*[dev] cap*/,
+                               float *cand_partial /*[dev] cap or NULL*/, int64_t cand_cap,
+                               unsigned long long *cand_count /*[dev] 1*/, unsigned long long *row_queue /*[dev] 1*/,
+                               int warps_per_cta, float *row_floor /*[dev] per left row id*/, int top_n,
+                               float floor_margin, float floor_margin_per_feature,
+                               const int32_t *self_rank /*[dev] per row id, or NULL*/, int seed, void *stream);
 
 /* ------------------------------------------------------------------------- *
  * K2, tile-centric form (csrc/sg_tiles.cu) — the default for L2-normalised non-negative matrices (K1 output).
@@ -348,6 +387,36 @@ int sg_rescore_refined(int64_t n_cand, const int32_t *cand_row, const int32_t *c
                        unsigned long long *refined_count /*[dev] 1 or NULL*/,
                        unsigned long long *mirror_count /*[dev] 1 or NULL*/,
                        int32_t *row_cnt /*[dev] or NULL*/, int64_t row_begin, void *stream);
+/* Top-n floor of the re-score (see sg_cossim_candidates_floor): a pair is kept only if its score is > keep_threshold
+ * AND >= row_floor[r].  Every row keeps at least top_n pairs at or above its floor, so the selection that follows
+ * returns the same output.  *floor_dropped [dev, zeroed, or NULL] += pairs above keep_threshold the floor removed.
+ * sg_rescore_refined_floor also raises the grouped bound's threshold to
+ * max(row_threshold[r], row_floor[r] - 1e-6 - (floor_margin + floor_margin_per_feature * row_len[r])), with the
+ * margins and row_len (sg_prune_rows' out_len) the candidates were generated with.  No mirror. */
+int sg_rescore_floor(int64_t n_cand, const int32_t *cand_row, const int32_t *cand_col,
+                     const int64_t *a_indptr, const int32_t *a_indices, const void *a_val,
+                     const int64_t *b_indptr, const int32_t *b_indices, const void *b_val, int dtype,
+                     double *score_out /*[dev] n_cand*/, double keep_threshold, int32_t *keep_row /*[dev] n_cand*/,
+                     int32_t *keep_col /*[dev] n_cand*/, unsigned long long *keep_count /*[dev] 1*/,
+                     int32_t *row_cnt /*[dev] or NULL*/, int64_t row_begin,
+                     const float *row_floor /*[dev] per left row id*/,
+                     unsigned long long *floor_dropped /*[dev] 1 or NULL*/, void *stream);
+int sg_rescore_refined_floor(int64_t n_cand, const int32_t *cand_row, const int32_t *cand_col,
+                             const float *cand_partial /*[dev] n_cand*/,
+                             const void *left_group_norms /*[dev] fp16[16] per left row id*/,
+                             const void *right_group_norms /*[dev] fp16[16] per right row id*/,
+                             const float *row_threshold /*[dev] per left row id*/,
+                             const int64_t *a_indptr, const int32_t *a_indices, const void *a_val,
+                             const int64_t *b_indptr, const int32_t *b_indices, const void *b_val, int dtype,
+                             double *score_out /*[dev] n_cand*/, double keep_threshold,
+                             int32_t *keep_row /*[dev] n_cand*/, int32_t *keep_col /*[dev] n_cand*/,
+                             unsigned long long *keep_count /*[dev] 1*/,
+                             unsigned long long *refined_count /*[dev] 1 or NULL*/,
+                             int32_t *row_cnt /*[dev] or NULL*/, int64_t row_begin,
+                             const float *row_floor /*[dev] per left row id*/,
+                             const int32_t *row_len /*[dev] per left row id*/, float floor_margin,
+                             float floor_margin_per_feature, unsigned long long *floor_dropped /*[dev] 1 or NULL*/,
+                             void *stream);
 
 /*
  * Per-row selection: keep score > threshold (strict, sg.py:729/:740), at most

@@ -45,6 +45,9 @@ TILE_MARGIN = 2e-5               # fp32 arithmetic of thresholds / norms and the
 TILE_MARGIN_PER_FEATURE = 3.1e-5  # a_q * w_q / 2^30 vs a * w: both weights rounded to nearest 2^-15 (<= 2^-15 + 2^-32)
 TILE_WARPS = int(os.environ.get("SG_B200_TILE_WARPS", "8"))
 SELECT_MODE = os.environ.get("SG_B200_SELECT", "rows").lower()      # "rows" (per-row ranking) | "sort" (global sorts)
+# top-n floor (cossim_topn's `floor`): "auto" | "1" | "0"; auto considers it from FLOOR_MIN_ROWS left rows on
+TOPN_FLOOR = {"1": True, "0": False}.get(os.environ.get("SG_B200_TOPN_FLOOR", "auto").lower(), "auto")
+FLOOR_MIN_ROWS = 65536
 
 
 def torch():
@@ -456,12 +459,36 @@ def prune_left(A, B, hrank, row_begin, row_end, threshold, margin, margin_per_fe
     return p_idx, p_val, p_len, p_thr, p_xp, p_xg
 
 
+def prune_left_floor(A, B, hrank, row_begin, row_end, threshold, margin, margin_per_feature, frac, row_floor):
+    """prune_left for the per-row thresholds max(threshold, row_floor[i] - 1e-6) (sg_prune_rows_floor)."""
+    t = require_cuda()
+    L = _lib.load()
+    df = feature_df(B)
+    p_idx = t.empty_like(A.d_indices)
+    p_val = t.empty_like(A.d_val32)
+    p_len = _empty(A.shape[0], t.int32, A.device)
+    p_thr = _empty(A.shape[0], t.float32, A.device)
+    p_xp = _empty(A.shape[0], t.float32, A.device)
+    p_xg = _empty(16 * A.shape[0], t.float16, A.device)
+    _lib.check(L.sg_prune_rows_floor(row_begin, row_end, _ptr(A.d_indptr), _ptr(A.d_indices), _ptr(A.d_val32),
+                                     _ptr(df), _ptr(hrank), float(B.norm_bound), float(frac), float(threshold),
+                                     _ptr(row_floor), float(margin), float(margin_per_feature), _ptr(p_idx),
+                                     _ptr(p_val), _ptr(p_len), _ptr(p_thr), _ptr(p_xp), _ptr(p_xg), _stream()))
+    LAUNCH_COUNTS["prune"] += 1
+    return p_idx, p_val, p_len, p_thr, p_xp, p_xg
+
+
 def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, warps=None, stats=None,
-                prune=None, acc=None, kernel=None):
+                prune=None, acc=None, kernel=None, floor=None):
     """C[i,:] = top_n{ j : A_i . B_j > threshold } for rows [row_begin,row_end) of A.
 
     Device counterpart of the whole block loop of StringGrouper._build_matches
     (string_grouper.py:734-750).  Returns DeviceMatches with absolute row ids.
+
+    `floor` (None = SG_B200_TOPN_FLOOR, default "auto"; True; False): the top-n floor of DESIGN.md §4, which bounds
+    the candidates of low thresholds by each row's top_n-th best score.  "auto" takes it only where the usual path
+    would not fit: top_n <= 32, threshold < 0.5, at least FLOOR_MIN_ROWS rows, and a sampled candidate count whose
+    24 bytes each exceed a quarter of device memory.  True needs top_n <= 32, threshold > 0 and non-negative operands.
     """
     t = require_cuda()
     L = _lib.load()
@@ -480,6 +507,24 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
     if n_rows == 0 or n_right == 0 or top_n <= 0 or A.nnz == 0 or B.nnz == 0:
         z32 = _empty(1, t.int32, dev)
         return DeviceMatches(shape, z32, z32, _empty(1, t.float64, dev), 0, 0)
+
+    if floor not in (None, "auto", True, False):
+        raise ValueError("floor must be None, 'auto', True or False, got %r" % (floor,))
+    floor_ok = top_n <= 32 and float(threshold) > 0.0 and A.nonneg and B.nonneg
+    if floor is None:       # the environment knob forces the floor only where it applies
+        floor = TOPN_FLOOR if (TOPN_FLOOR is not True or floor_ok) else False
+    if floor is True:
+        if not floor_ok:
+            raise ValueError("the top-n floor needs top_n <= 32, min_similarity > 0 and non-negative matrices")
+        if (kernel or "row").lower() != "row":
+            raise ValueError("the top-n floor runs on the row kernel only")
+    if floor is True or (floor == "auto" and floor_ok and float(threshold) < 0.5 and n_rows >= FLOOR_MIN_ROWS):
+        out = _cossim_topn_floor(A, B, top_n, float(threshold), row_begin, row_end, tile_w, stats, prune, acc,
+                                 decide=floor == "auto")
+        if out is not None:
+            return out
+    if stats is not None:
+        stats["topn_floor"] = False
 
     mark(stats, "k2_start")
     scale = A.norm_bound * B.norm_bound
@@ -773,6 +818,228 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
         if use_tiles:
             stats["stage_bytes"] = tiles["stage_bytes"]
 
+    return _select_topn(cand_row, cand_col, score, n_cand, row_cnt, max_row_cnt, row_begin, n_rows, top_n, threshold,
+                        shape, stats)
+
+
+def _cossim_topn_floor(A, B, top_n, threshold, row_begin, row_end, tile_w, stats, prune, acc, decide):
+    """cossim_topn with the top-n floor (DESIGN.md §4): row kernel, full product (no triangle), 8 warps per CTA.
+
+    floor[r] is a proven lower bound of the exact score of row r's top_n-th best pair, raised by the candidates
+    kernel as it finds pairs.  A self-match first walks every row's own column-tile group (the seed, where clusters of
+    identical names set high floors at once), prunes the left rows again for max(threshold, floor), then walks the
+    other groups.  The re-score keeps only pairs at or above the floor, which changes no output.  With `decide` the
+    floor is taken only if the sampled candidate count of the usual path needs more than a quarter of device memory;
+    otherwise None is returned and the caller runs the usual path."""
+    t = require_cuda()
+    L = _lib.load()
+    n_left, n_right = A.shape[0], B.shape[0]
+    n_rows = row_end - row_begin
+    dev = A.device
+    dt = _lib.SG_DTYPE_F32 if A.dtype == np.float32 else _lib.SG_DTYPE_F64
+    scale = A.norm_bound * B.norm_bound
+    margin = CAND_MARGIN * max(scale, 1.0)
+    thr_c = max(threshold - margin, 0.0)
+    acc = (acc or ACC_DTYPE).lower()
+    if acc not in ("u16", "f32"):
+        raise ValueError("accumulator dtype must be 'u16' or 'f32', got %r" % (acc,))
+    if scale > 1.0 + 1e-6 or thr_c < 0.05:
+        acc = "f32"
+    acc_code = _lib.SG_ACC_U16 if acc == "u16" else _lib.SG_ACC_F32
+    margin_pf = U16_MARGIN_PER_FEATURE if acc == "u16" else 0.0
+    level = PRUNE_FRAC if prune is None else float(prune)
+    if thr_c <= 0.0:
+        level = 0.0
+    warps = 8                                   # the floor variant of the candidates kernel is built for 8 warps
+    tile_w, _ = pick_tile(n_right, tile_w, warps, 2 if acc == "u16" else 4, n_left=n_rows)
+    while (-(-n_right // tile_w)) * (B.shape[1] + 1) > MAX_BUCKETS and tile_w < 32768:
+        tile_w *= 2
+    hrank, perm_b, rank_b, bucket_dir, bucket_maxw, post, T, tile_bound = right_side(B, tile_w)
+    tiles_per_group = max(64, int(GROUP_BYTES // max(4 * B.nnz / T, 1)) // 64 * 64)
+    # a self-match (any row range) seeds the floors from each row's own column-tile group
+    self_match = A is B
+    if self_match and row_begin == 0 and row_end == n_left:
+        perm_a = perm_b
+    else:
+        perm_a, _ = row_order(A, hrank, row_begin, row_end, want_rank=False)
+    self_rank = rank_b if self_match else None
+    total_mem = t.cuda.get_device_properties(dev).total_memory
+    refine = REFINE and acc == "u16" and margin_pf > 0.0
+    counters = t.zeros(4, dtype=t.int64, device=dev)   # [0] candidates / kept, [1] queue, [2] refined, [3] dropped
+    c_count = ctypes.c_void_p(counters.data_ptr())
+    c_queue = ctypes.c_void_p(counters.data_ptr() + 8)
+    c_refined = ctypes.c_void_p(counters.data_ptr() + 16)
+    c_dropped = ctypes.c_void_p(counters.data_ptr() + 24)
+    dummy = _empty(1, t.int32, dev)
+    sample = stride = None
+    if n_rows >= 65536 and not os.environ.get("SG_B200_CAND_CAP"):
+        stride = max(64, n_rows // 8192)
+        sample = perm_a[:n_rows:stride].contiguous()
+
+    def pruned(row_floor=None):
+        if level <= 0.0 and margin_pf <= 0.0:
+            return (A.d_indices, A.d_val32, None, None, None, None)
+        if row_floor is None:
+            return prune_left(A, B, hrank, row_begin, row_end, threshold, margin, margin_pf, level)
+        return prune_left_floor(A, B, hrank, row_begin, row_end, threshold, margin, margin_pf, level, row_floor)
+
+    arrays = pruned()
+    mark(stats, "right_side")
+    if decide and sample is None:
+        return None
+    if decide:
+        # the usual path's sample at its first pruning level (full product): its candidates at 24 B each
+        l_idx, l_val, l_len, l_thr, l_xp, _ = arrays
+        counters.zero_()
+        _lib.check(L.sg_cossim_candidates(
+            _ptr(A.d_indptr), _ptr(l_len), _ptr(l_idx), _ptr(l_val), row_begin, row_begin + int(sample.numel()),
+            _ptr(sample), n_right, A.shape[1], _ptr(bucket_dir), _ptr(bucket_maxw), _ptr(post), _ptr(perm_b), tile_w,
+            acc_code, max(B.norm_bound, 1.0), thr_c, _ptr(l_thr), _ptr(l_xp), _ptr(tile_bound), tiles_per_group,
+            None, None, _ptr(dummy), _ptr(dummy), None, 0, c_count, c_queue, warps, _stream()))
+        LAUNCH_COUNTS["candidates"] += 1
+        est_usual = int(counters[0].item()) * stride
+        if stats is not None:
+            stats["n_candidates_estimate_usual"] = est_usual
+        if est_usual * 24 <= total_mem // 4:
+            return None
+    floor_buf = t.zeros(n_left, dtype=t.float32, device=dev)
+
+    def launch(perm, n, arrs, row_buf, col_buf, part_buf, capacity, seed):
+        l_idx, l_val, l_len, l_thr, l_xp, _ = arrs
+        counters.zero_()
+        _lib.check(L.sg_cossim_candidates_floor(
+            _ptr(A.d_indptr), _ptr(l_len), _ptr(l_idx), _ptr(l_val), row_begin, row_begin + n, _ptr(perm), n_right,
+            A.shape[1], _ptr(bucket_dir), _ptr(bucket_maxw), _ptr(post), _ptr(perm_b), tile_w, acc_code,
+            max(B.norm_bound, 1.0), thr_c, _ptr(l_thr), _ptr(l_xp), _ptr(tile_bound), tiles_per_group, _ptr(row_buf),
+            _ptr(col_buf), _ptr(part_buf), capacity, c_count, c_queue, warps, _ptr(floor_buf), top_n, margin,
+            margin_pf, _ptr(self_rank), 1 if seed else 0, _stream()))
+        LAUNCH_COUNTS["candidates"] += 1
+        return int(counters[0].item())
+
+    def collect(perm, n, arrs, seed, cap):
+        """candidates of the rows `perm`; a launch that overflowed its buffer is repeated with the count it found
+        (the floors it raised only lower the count of the repeat)"""
+        for _ in range(3):
+            row_buf, col_buf = _empty(cap, t.int32, dev), _empty(cap, t.int32, dev)
+            part_buf = _empty(cap, t.float32, dev) if refine else None
+            n_c = launch(perm, n, arrs, row_buf, col_buf, part_buf, cap, seed)
+            if n_c <= cap:
+                return row_buf, col_buf, part_buf, n_c
+            del row_buf, col_buf, part_buf
+            if n_c * 24 > total_mem // 2:
+                raise OverflowError("%d candidate pairs do not fit the candidate buffer even with the top-n floor; "
+                                    "raise min_similarity or split the input" % n_c)
+            cap = n_c
+        raise OverflowError("candidate buffer overflow")
+
+    row_cnt = t.zeros(n_rows + 1, dtype=t.int32, device=dev)
+    totals = {"kept": 0, "refined": 0, "dropped": 0}
+
+    def rescore(cand, arrs):
+        """exact scores; keeps the pairs > threshold and >= floor (survivors, buffers of their own size)"""
+        row_buf, col_buf, part_buf, n_c = cand
+        l_idx, l_val, l_len, l_thr, l_xp, l_xg = arrs
+        score = _empty(n_c, t.float64, dev)
+        keep_row = _empty(n_c, t.int32, dev)
+        keep_col = _empty(n_c, t.int32, dev)
+        counters.zero_()
+        if refine and part_buf is not None and l_xg is not None:
+            _lib.check(L.sg_rescore_refined_floor(
+                n_c, _ptr(row_buf), _ptr(col_buf), _ptr(part_buf), _ptr(l_xg), _ptr(B._heavy_groups), _ptr(l_thr),
+                _ptr(A.d_indptr), _ptr(A.d_indices), _ptr(A.d_val), _ptr(B.d_indptr), _ptr(B.d_indices),
+                _ptr(B.d_val), dt, _ptr(score), threshold, _ptr(keep_row), _ptr(keep_col), c_count, c_refined,
+                _ptr(row_cnt), row_begin, _ptr(floor_buf), _ptr(l_len), margin, margin_pf, c_dropped, _stream()))
+        else:
+            _lib.check(L.sg_rescore_floor(
+                n_c, _ptr(row_buf), _ptr(col_buf), _ptr(A.d_indptr), _ptr(A.d_indices), _ptr(A.d_val),
+                _ptr(B.d_indptr), _ptr(B.d_indices), _ptr(B.d_val), dt, _ptr(score), threshold, _ptr(keep_row),
+                _ptr(keep_col), c_count, _ptr(row_cnt), row_begin, _ptr(floor_buf), c_dropped, _stream()))
+        LAUNCH_COUNTS["rescore"] += 1
+        head = counters.cpu().numpy()
+        n_keep = int(head[0])
+        totals["kept"] += n_keep
+        totals["refined"] += int(head[2])
+        totals["dropped"] += int(head[3])
+        return keep_row[:n_keep].clone(), keep_col[:n_keep].clone(), score[:n_keep].clone(), n_keep
+
+    kept = []
+    n_seed = 0
+    base_cap = min(96 * n_rows + (1 << 22), CAND_CHUNK)
+    if self_match:
+        cand = collect(perm_a, n_rows, arrays, True, base_cap)
+        n_seed = cand[3]
+        kept.append(rescore(cand, arrays))
+        del cand
+        if arrays[2] is not None:
+            arrays = pruned(floor_buf)      # per-row thresholds max(threshold, floor) for the other groups
+        mark(stats, "floor_seed")
+    # The other groups (every group without a seed), in row chunks whose candidates fit CAND_CHUNK entries, sized
+    # from a sample of the rows or from a first launch over all of them that overflowed its buffer.
+    est, first = None, None
+    if sample is not None:
+        est = launch(sample, int(sample.numel()), arrays, dummy, dummy, None, 0, False) * stride
+    else:
+        bufs = (_empty(base_cap, t.int32, dev), _empty(base_cap, t.int32, dev),
+                _empty(base_cap, t.float32, dev) if refine else None)
+        n0 = launch(perm_a, n_rows, arrays, bufs[0], bufs[1], bufs[2], base_cap, False)
+        if n0 <= base_cap:
+            first = bufs + (n0,)
+        else:
+            est = n0
+        del bufs
+    n_chunks = 1 if est is None else max(1, -(-int(1.3 * est) // CAND_CHUNK))
+    rows_per_chunk = -(-n_rows // n_chunks)
+    n_main = 0
+    for lo in range(0, n_rows, rows_per_chunk):
+        hi = min(lo + rows_per_chunk, n_rows)
+        if first is not None:
+            cand, first = first, None
+        else:
+            perm_chunk = perm_a if (lo == 0 and hi == n_rows) else perm_a[lo:hi]
+            cap = base_cap if est is None else min(max(int(1.3 * est * (hi - lo) / n_rows) + (1 << 22), 1 << 22),
+                                                   1 << 31)
+            cand = collect(perm_chunk, hi - lo, arrays, False, cap)
+        n_main += cand[3]
+        kept.append(rescore(cand, arrays))
+        del cand
+    mark(stats, "candidates")
+    counters.zero_()
+    _lib.check(L.sg_row_count_max(n_rows, _ptr(row_cnt), c_queue, _stream()))
+    max_row_cnt = int(counters[1].item())
+    n_keep = sum(k[3] for k in kept)
+    if n_keep:
+        cand_row = t.cat([k[0] for k in kept])
+        cand_col = t.cat([k[1] for k in kept])
+        score = t.cat([k[2] for k in kept])
+    else:
+        cand_row, cand_col, score = _empty(1, t.int32, dev), _empty(1, t.int32, dev), _empty(1, t.float64, dev)
+    del kept
+    mark(stats, "rescore")
+    if stats is not None:
+        stats["topn_floor"] = True
+        stats["prune"], stats["acc"], stats["kernel"] = level, acc, "row"
+        stats["n_candidates_estimate"] = est
+        stats["n_candidates_seed"], stats["n_candidates_main"] = n_seed, n_main
+        stats["n_candidates"] = n_seed + n_main
+        stats["n_floor_dropped"] = totals["dropped"]
+        stats["n_survivors"] = n_keep
+        stats["n_above_threshold"] = n_keep + totals["dropped"]
+        if refine:
+            stats["n_refined"] = totals["refined"]
+        stats["triangle"] = False
+        stats["n_row_chunks"] = n_chunks
+        stats["tile_w"], stats["warps"], stats["n_tiles"] = tile_w, warps, T
+        stats["tiles_per_group"] = tiles_per_group
+    return _select_topn(cand_row, cand_col, score, n_keep, row_cnt, max_row_cnt, row_begin, n_rows, top_n, threshold,
+                        (n_left, n_right), stats)
+
+
+def _select_topn(cand_row, cand_col, score, n_cand, row_cnt, max_row_cnt, row_begin, n_rows, top_n, threshold, shape,
+                 stats):
+    """Top-n per row of the re-scored survivors (row ids absolute, `row_cnt` survivors per row of the range)."""
+    t = torch()
+    L = _lib.load()
+    dev = cand_row.device
     out_indptr = _empty(n_rows + 1, t.int64, dev)
     out_row = _empty(n_cand, t.int32, dev)
     out_col = _empty(n_cand, t.int32, dev)

@@ -53,10 +53,15 @@ SIGNATURES = {
     "sg_postings_build": (_i32, [_i64, _i64, _i64, _p, _p, _p, _p, _i32, _i64, _f32, _p, _p, _p, _p, _p, _sz, _p]),
     "sg_feature_df": (_i32, [_i64, _i64, _p, _p, _p, _p]),
     "sg_prune_rows": (_i32, [_i64, _i64, _p, _p, _p, _p, _p, _f32, _f32, _f32, _f32, _f32, _p, _p, _p, _p, _p, _p, _p]),
+    "sg_prune_rows_floor": (_i32, [_i64, _i64, _p, _p, _p, _p, _p, _f32, _f32, _f32, _p, _f32, _f32, _p, _p, _p, _p,
+                                   _p, _p, _p]),
     "sg_heavy_norms": (_i32, [_i64, _i64, _p, _p, _p, _p, _p, _p, _p]),
     "sg_tile_bounds": (_i32, [_i64, _p, _p, _i32, _p, _p]),
     "sg_cossim_candidates": (_i32, [_p, _p, _p, _p, _i64, _i64, _p, _i64, _i64, _p, _p, _p, _p, _i32, _i32, _f32,
                                     _f32, _p, _p, _p, _i64, _p, _p, _p, _p, _p, _i64, _p, _p, _i32, _p]),
+    "sg_cossim_candidates_floor": (_i32, [_p, _p, _p, _p, _i64, _i64, _p, _i64, _i64, _p, _p, _p, _p, _i32, _i32,
+                                          _f32, _f32, _p, _p, _p, _i64, _p, _p, _p, _i64, _p, _p, _i32, _p, _i32,
+                                          _f32, _f32, _p, _i32, _p]),
     "sg_tiles_tile_w": (_i32, []),
     "sg_tiles_max_cols": (_i64, []),
     "sg_tiles_blob_bound": (_i64, [_i64, _i64, _i64]),
@@ -74,6 +79,10 @@ SIGNATURES = {
     "sg_rescore": (_i32, [_i64, _p, _p, _p, _p, _p, _p, _p, _p, _i32, _p, _f64, _p, _p, _p, _p, _p, _i64, _p]),
     "sg_rescore_refined": (_i32, [_i64, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i32, _p, _f64, _p, _p, _p, _p,
                                   _p, _p, _i64, _p]),
+    "sg_rescore_floor": (_i32, [_i64, _p, _p, _p, _p, _p, _p, _p, _p, _i32, _p, _f64, _p, _p, _p, _p, _i64, _p, _p,
+                                _p]),
+    "sg_rescore_refined_floor": (_i32, [_i64, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i32, _p, _f64, _p, _p,
+                                        _p, _p, _p, _i64, _p, _p, _f32, _f32, _p, _p]),
     "sg_topn_rows_cap": (_i32, []),
     "sg_row_count_max": (_i32, [_i64, _p, _p, _p]),
     "sg_topn_select_rows_workspace_bytes": (_sz, [_i64, _i64]),

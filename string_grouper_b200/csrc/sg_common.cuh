@@ -46,6 +46,10 @@ struct Arena {
 
 constexpr unsigned FULL = 0xffffffffu;
 
+// Top-n floor (sg_cossim_candidates_floor): a pair must stay a candidate when its exact score can be >= floor[row]
+// (ties at the cut are resolved by column), so the thresholds derived from a floor f are those of "score > f - FLOOR_EPS".
+constexpr float FLOOR_EPS = 1e-6f;
+
 __device__ __forceinline__ int lane_id() { return threadIdx.x & 31; }
 
 }  // namespace sg

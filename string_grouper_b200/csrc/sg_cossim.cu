@@ -256,19 +256,59 @@ __device__ __forceinline__ void apply_buckets(AccT *__restrict__ acc, const uint
 // out of the block-max ballot; in the tile holding the rank the columns below it are not reported.
 // `group_items` (with diag_rank): exclusive offsets of the work items per column-tile group (diag_items_kernel), so
 // that no item is handed out whose row has no tile at or above its rank in the group.
-template <int NW, typename AccT>
-__global__ void __launch_bounds__(NW * 32, min_ctas(NW))
-cossim_candidates_kernel(const int64_t *__restrict__ a_indptr, const int32_t *__restrict__ a_len,
-                         const int32_t *__restrict__ a_idx, const float *__restrict__ a_val, int64_t row_begin,
-                         int64_t row_end, const int32_t *__restrict__ perm_a, int64_t n_right,
-                         const int2 *__restrict__ bdir, const uint32_t *__restrict__ maxw_h,
-                         const uint32_t *__restrict__ post, const int32_t *__restrict__ perm_b, int Tp, int W,
-                         int64_t T, int64_t tiles_per_group, float a_scale, float thr_all,
-                         const float *__restrict__ thr_row, const float *__restrict__ xp_norm,
-                         const float *__restrict__ tile_bound, const int32_t *__restrict__ diag_rank,
-                         const unsigned long long *__restrict__ group_items, int32_t *__restrict__ cand_row,
-                         int32_t *__restrict__ cand_col, float *__restrict__ cand_partial, unsigned long long cap,
-                         unsigned long long *__restrict__ cand_count, unsigned long long *__restrict__ row_queue) {
+//
+// Top-n floor (cossim_candidates_floor_kernel, top_n <= 32, non-negative weights): floor[row] is a proven lower bound
+// of the exact score of the row's top_n-th best pair; it only rises.  A pair whose exact score is below it cannot be
+// in the row's output, so the candidate threshold of the row becomes max(thr_row, floor - E_r - FLOOR_EPS), read again
+// at every 64-tile batch (block-max ballot and sweep).  E_r = margin + margin_pf * kept features bounds how far the
+// accumulated partial p^ can differ from the kept-feature product x_S.y in EITHER direction (the fp16 posting weights
+// and the fixed-point / fp32 roundings are symmetric; the same constants give thr_row), and x_S.y <= exact for
+// non-negative weights.  So p^ - E_r (rounded down) is a lower bound of the exact score of every reported pair: the
+// warp keeps the best 32 of them per work item, one per lane, and once top_n exist publishes the top_n-th with
+// atomicMax (non-negative floats order like their bits).  The pairs of one item are distinct columns.
+// Self-match (`self_rank` = every row's position in the common processing order): `seed` = 1 walks only the row's own
+// column-tile group, starting at the 64-tile batch that holds the row (clusters of identical names sit next to each
+// other in that order, so this is where floors rise first); `seed` = 0 walks every other group.
+struct FloorArgs {
+    float *floor;
+    const int32_t *self_rank;
+    int seed, top_n;
+    float margin, margin_pf;
+};
+
+// kept: the best 32 values so far, descending over the lanes; x: one new value per lane.  Sort x ascending, the lane-wise
+// maxima are the best 32 of the union as a bitonic sequence, five merge stages sort them (as sel_rows_kernel does).
+__device__ __forceinline__ void floor_merge(float &kept, float x, int lane) {
+#pragma unroll
+    for (int k = 2; k <= 32; k <<= 1) {
+#pragma unroll
+        for (int j = k >> 1; j > 0; j >>= 1) {
+            const float o = __shfl_xor_sync(FULL, x, j);
+            x = (((lane & k) == 0) == ((lane & j) == 0)) ? fminf(x, o) : fmaxf(x, o);
+        }
+    }
+    kept = fmaxf(kept, x);
+#pragma unroll
+    for (int j = 16; j > 0; j >>= 1) {
+        const float o = __shfl_xor_sync(FULL, kept, j);
+        kept = (lane & j) == 0 ? fmaxf(kept, o) : fminf(kept, o);
+    }
+}
+
+template <int NW, typename AccT, bool FLOOR>
+__device__ __forceinline__ void
+candidates_body(const int64_t *__restrict__ a_indptr, const int32_t *__restrict__ a_len,
+                const int32_t *__restrict__ a_idx, const float *__restrict__ a_val, int64_t row_begin,
+                int64_t row_end, const int32_t *__restrict__ perm_a, int64_t n_right,
+                const int2 *__restrict__ bdir, const uint32_t *__restrict__ maxw_h,
+                const uint32_t *__restrict__ post, const int32_t *__restrict__ perm_b, int Tp, int W,
+                int64_t T, int64_t tiles_per_group, float a_scale, float thr_all,
+                const float *__restrict__ thr_row, const float *__restrict__ xp_norm,
+                const float *__restrict__ tile_bound, const int32_t *__restrict__ diag_rank,
+                const unsigned long long *__restrict__ group_items, int32_t *__restrict__ cand_row,
+                int32_t *__restrict__ cand_col, float *__restrict__ cand_partial, unsigned long long cap,
+                unsigned long long *__restrict__ cand_count, unsigned long long *__restrict__ row_queue,
+                const FloorArgs &fa) {
     typedef AccOps<AccT> Ops;
     typedef typename Ops::val_t val_t;
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -287,8 +327,11 @@ cossim_candidates_kernel(const int64_t *__restrict__ a_indptr, const int32_t *__
     // large the right matrix is.  tiles_per_group is a multiple of 64.
     const int64_t n_rows = row_end - row_begin;
     const int64_t n_groups = (T + tiles_per_group - 1) / tiles_per_group;
-    const unsigned long long n_items =
+    unsigned long long n_items =
         group_items ? group_items[n_groups] : (unsigned long long)n_rows * (unsigned long long)n_groups;
+    if constexpr (FLOOR) {
+        if (fa.self_rank) n_items = (unsigned long long)n_rows * (unsigned long long)(fa.seed ? 1 : n_groups - 1);
+    }
     const int n_tiles = (int)T;
     int64_t group = 0;          // with group_items: items arrive in increasing order, so the group only moves forward
     for (;;) {
@@ -305,10 +348,26 @@ cossim_candidates_kernel(const int64_t *__restrict__ a_indptr, const int32_t *__
             ridx = (int64_t)(item % (unsigned long long)n_rows);
         }
         const int64_t row = perm_a ? perm_a[ridx] : row_begin + ridx;   // processing order: neighbours share buckets
+        int own_batch = 0;      // floor seed: the walk starts at the 64-tile batch holding the row
+        if constexpr (FLOOR) {
+            if (fa.self_rank) {
+                const int64_t pos = fa.self_rank[row];
+                const int64_t own = pos / (tiles_per_group * W);
+                if (fa.seed) {
+                    group = own;
+                    own_batch = (int)((pos / W - own * tiles_per_group) >> 6);
+                } else if (group >= own) {
+                    ++group;
+                }
+            }
+        }
         const int64_t p0 = a_indptr[row];
         const int nf = a_len ? a_len[row] : (int)(a_indptr[row + 1] - p0);
         if (nf == 0) continue;
-        const float thr_r = thr_row ? thr_row[row] : thr_all;
+        float thr_r = thr_row ? thr_row[row] : thr_all;
+        // floor: E_r rounded up, the best 32 lower bounds of this item (descending over the lanes), the floor last seen
+        float e_r = 0.f, kept = 0.f, floor_seen = 0.f;
+        if constexpr (FLOOR) e_r = __fmaf_ru(fa.margin_pf, (float)nf, fa.margin);
         const float xp = xp_norm ? xp_norm[row] : 0.f;
         // tile ids, directory slots (T * V1 < 2^31, checked by sg_postings_build) and positions fit 32 bits
         const int t_begin = (int)(group * tiles_per_group);
@@ -333,7 +392,17 @@ cossim_candidates_kernel(const int64_t *__restrict__ a_indptr, const int32_t *__
         // fp16 arithmetic of the bound: one rounding of at most 2^-11 (values below 2) per kept feature
         const float slack = 5e-4f * (float)nk + 1e-4f;
 
-        for (int tb = tb_begin; tb < t_end; tb += 64) {
+        for (int tb0 = tb_begin; tb0 < t_end; tb0 += 64) {
+            int tb = tb0;
+            if constexpr (FLOOR) {
+                tb += own_batch * 64;           // batches of the group in rotated order
+                if (tb >= t_end) tb -= (t_end - tb_begin + 63) / 64 * 64;
+                const float f = __shfl_sync(FULL, __ldcg(fa.floor + row), 0);
+                if (f > floor_seen) {
+                    floor_seen = f;
+                    thr_r = fmaxf(thr_r, __fsub_rd(__fsub_rd(f, e_r), FLOOR_EPS));
+                }
+            }
             // ---- bounds of tiles tb + 2*lane and tb + 2*lane + 1 (tiles wholly below the rank are not taken)
             unsigned m_even, m_odd;
             const int t0 = tb + 2 * lane;
@@ -416,6 +485,21 @@ cossim_candidates_kernel(const int64_t *__restrict__ a_indptr, const int32_t *__
                                 if (below > 0) m = below >= Ops::PER16 ? 0u : m & (~0u << below);
                             }
                         }
+                        if constexpr (FLOOR) {
+                            // the lane's best new lower bound p^ - E_r joins the item's best 32
+                            float best = 0.f;
+                            for (unsigned mm = m; mm; mm &= mm - 1) best = fmaxf(best, Ops::value(v, __ffs(mm) - 1));
+                            const float lb = fmaxf(__fsub_rd(best, e_r), 0.f);
+                            if (__any_sync(FULL, lb > __shfl_sync(FULL, kept, fa.top_n - 1))) {
+                                floor_merge(kept, lb, lane);
+                                const float kth = __shfl_sync(FULL, kept, fa.top_n - 1);
+                                if (kth > floor_seen) {
+                                    floor_seen = kth;
+                                    if (lane == 0) atomicMax(reinterpret_cast<int *>(fa.floor + row), __float_as_int(kth));
+                                    thr_r = fmaxf(thr_r, __fsub_rd(__fsub_rd(kth, e_r), FLOOR_EPS));
+                                }
+                            }
+                        }
                         if (__any_sync(FULL, m != 0)) {
                             const int cnt = __popc(m);
                             int incl = cnt;
@@ -448,6 +532,34 @@ cossim_candidates_kernel(const int64_t *__restrict__ a_indptr, const int32_t *__
         }
     }
 }
+
+#define SG_CAND_PARAMS                                                                                              \
+    const int64_t *__restrict__ a_indptr, const int32_t *__restrict__ a_len, const int32_t *__restrict__ a_idx,     \
+        const float *__restrict__ a_val, int64_t row_begin, int64_t row_end, const int32_t *__restrict__ perm_a,    \
+        int64_t n_right, const int2 *__restrict__ bdir, const uint32_t *__restrict__ maxw_h,                        \
+        const uint32_t *__restrict__ post, const int32_t *__restrict__ perm_b, int Tp, int W, int64_t T,            \
+        int64_t tiles_per_group, float a_scale, float thr_all, const float *__restrict__ thr_row,                   \
+        const float *__restrict__ xp_norm, const float *__restrict__ tile_bound,                                    \
+        const int32_t *__restrict__ diag_rank, const unsigned long long *__restrict__ group_items,                  \
+        int32_t *__restrict__ cand_row, int32_t *__restrict__ cand_col, float *__restrict__ cand_partial,           \
+        unsigned long long cap, unsigned long long *__restrict__ cand_count,                                        \
+        unsigned long long *__restrict__ row_queue
+#define SG_CAND_ARGS                                                                                              \
+    a_indptr, a_len, a_idx, a_val, row_begin, row_end, perm_a, n_right, bdir, maxw_h, post, perm_b, Tp, W, T,     \
+        tiles_per_group, a_scale, thr_all, thr_row, xp_norm, tile_bound, diag_rank, group_items, cand_row,        \
+        cand_col, cand_partial, cap, cand_count, row_queue
+
+template <int NW, typename AccT>
+__global__ void __launch_bounds__(NW * 32, min_ctas(NW)) cossim_candidates_kernel(SG_CAND_PARAMS) {
+    candidates_body<NW, AccT, false>(SG_CAND_ARGS, FloorArgs{});
+}
+
+template <int NW, typename AccT>
+__global__ void __launch_bounds__(NW * 32, min_ctas(NW)) cossim_candidates_floor_kernel(SG_CAND_PARAMS, FloorArgs fa) {
+    candidates_body<NW, AccT, true>(SG_CAND_ARGS, fa);
+}
+#undef SG_CAND_PARAMS
+#undef SG_CAND_ARGS
 
 // Work items of the triangle.  A row has work in the groups from the one holding its rank on, so group g needs the
 // items ridx < last[g] = 1 + the largest ridx whose first group is <= g (a prefix of the launch; exact when the ranks
@@ -611,6 +723,27 @@ __device__ __forceinline__ void keep_pairs(bool keep, bool mir, int32_t r, int32
     }
 }
 
+// Top-n floor of the re-score (sg_rescore_floor / sg_rescore_refined_floor): a pair above the threshold is kept only
+// if its exact score is >= floor[r] (at least top_n pairs of the row score that much, so it changes no output);
+// `dropped` (optional) counts the pairs above the threshold the floor removed.  The refined kernel's grouped bound
+// tests against max(row_threshold[r], floor[r] - FLOOR_EPS - E_r), E_r = margin + margin_pf * row_len[r] as in the
+// candidates kernel.
+struct RescoreFloor {
+    const float *floor;
+    const int32_t *row_len;
+    float margin, margin_pf;
+    unsigned long long *dropped;
+};
+
+__device__ __forceinline__ bool floor_keep(bool keep, int32_t r, double sc, const RescoreFloor &rf) {
+    const bool drop = keep && sc < (double)rf.floor[r];
+    if (rf.dropped) {
+        const unsigned m = __ballot_sync(FULL, drop);
+        if (m && lane_id() == __ffs(m) - 1) atomicAdd(rf.dropped, (unsigned long long)__popc(m));
+    }
+    return keep && !drop;
+}
+
 template <typename T, int VEC>
 __global__ void __launch_bounds__(256, 8) rescore_kernel(int64_t n, const int32_t *__restrict__ cr, const int32_t *__restrict__ cc,
                                const int64_t *__restrict__ a_indptr, const int32_t *__restrict__ a_idx,
@@ -619,7 +752,7 @@ __global__ void __launch_bounds__(256, 8) rescore_kernel(int64_t n, const int32_
                                double *__restrict__ out, double keep_thr, int32_t *__restrict__ keep_row,
                                int32_t *__restrict__ keep_col, unsigned long long *__restrict__ keep_count,
                                unsigned long long *__restrict__ mirror_count, int32_t *__restrict__ row_cnt,
-                               int64_t row_begin) {
+                               int64_t row_begin, RescoreFloor rf) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     int32_t r = 0, c = 0;
     double sc = 0.0;
@@ -635,6 +768,7 @@ __global__ void __launch_bounds__(256, 8) rescore_kernel(int64_t n, const int32_
         keep = keep_count && sc > keep_thr;
     }
     if (!keep_count) return;
+    if (rf.floor) keep = floor_keep(keep, r, sc, rf);
     keep_pairs(keep, keep && mirror_count && r != c, r, c, sc, threadIdx.x & 31, keep_row, keep_col, out, keep_count,
                mirror_count, row_cnt, row_begin);
 }
@@ -672,7 +806,7 @@ rescore_refined_kernel(int64_t n, const int32_t *__restrict__ cr, const int32_t 
                        double keep_thr, int32_t *__restrict__ keep_row, int32_t *__restrict__ keep_col,
                        unsigned long long *__restrict__ keep_count, unsigned long long *__restrict__ refined_count,
                        unsigned long long *__restrict__ mirror_count, int32_t *__restrict__ row_cnt,
-                       int64_t row_begin) {
+                       int64_t row_begin, RescoreFloor rf) {
     __shared__ uint16_t live[REFINE_CHUNK];
     __shared__ int n_live;
     const int lane = threadIdx.x & 31;
@@ -684,7 +818,12 @@ rescore_refined_kernel(int64_t n, const int32_t *__restrict__ cr, const int32_t 
         bool pass = false;
         if (i < n) {
             const int32_t r = cr[i], c = cc[i];
-            pass = partial[i] + group_dot(xg + 2 * (int64_t)r, yg + 2 * (int64_t)c) > thr_row[r];
+            float thr = thr_row[r];
+            if (rf.floor) {
+                const float e_r = __fmaf_ru(rf.margin_pf, (float)rf.row_len[r], rf.margin);
+                thr = fmaxf(thr, __fsub_rd(__fsub_rd(rf.floor[r], e_r), FLOOR_EPS));
+            }
+            pass = partial[i] + group_dot(xg + 2 * (int64_t)r, yg + 2 * (int64_t)c) > thr;
         }
         const unsigned m = __ballot_sync(FULL, pass);
         if (m) {
@@ -712,6 +851,7 @@ rescore_refined_kernel(int64_t n, const int32_t *__restrict__ cr, const int32_t 
                                             b_indptr[c + 1]);
             keep = sc > keep_thr;
         }
+        if (rf.floor) keep = floor_keep(keep, r, sc, rf);
         keep_pairs(keep, keep && mirror_count && r != c, r, c, sc, lane, keep_row, keep_col, out, keep_count,
                    mirror_count, row_cnt, row_begin);
     }
@@ -898,7 +1038,7 @@ int sg_postings_build(int64_t n_rows, int64_t n_cols, int64_t nnz, const int64_t
 
 }  // extern "C"
 
-template <int NW, typename AccT>
+template <int NW, typename AccT, bool FLOOR>
 static int launch_candidates(const int64_t *a_indptr, const int32_t *a_len, const int32_t *a_indices,
                              const float *a_val32, int64_t row_begin, int64_t row_end, const int32_t *perm_a,
                              int64_t n_right, int64_t n_cols, const void *bucket_dir, const void *bucket_maxw,
@@ -908,10 +1048,12 @@ static int launch_candidates(const int64_t *a_indptr, const int32_t *a_len, cons
                              const int32_t *diag_rank, unsigned long long *group_items,
                              int32_t *cand_row, int32_t *cand_col, float *cand_partial,
                              int64_t cand_cap, unsigned long long *cand_count, unsigned long long *row_queue,
-                             int n_sm, cudaStream_t st) {
+                             int n_sm, cudaStream_t st, const FloorArgs &fa) {
     const size_t smem = (size_t)NW * tile_w * sizeof(AccT);
-    SG_CUDA_TRY(cudaFuncSetAttribute(cossim_candidates_kernel<NW, AccT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     (int)smem));
+    const void *kern;
+    if constexpr (FLOOR) kern = (const void *)cossim_candidates_floor_kernel<NW, AccT>;
+    else kern = (const void *)cossim_candidates_kernel<NW, AccT>;
+    SG_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const int64_t T = sg_num_tiles(n_right, tile_w);
     const int64_t n_rows = row_end - row_begin;
     if (diag_rank) {
@@ -924,34 +1066,37 @@ static int launch_candidates(const int64_t *a_indptr, const int32_t *a_len, cons
         SG_LAUNCH_CHECK();
     }
     int per_sm = 1;
-    SG_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, cossim_candidates_kernel<NW, AccT>, NW * 32,
-                                                              smem));
+    SG_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, NW * 32, smem));
     if (per_sm < 1) per_sm = 1;
     int64_t ctas = (n_rows + NW - 1) / NW;
     if (ctas > (int64_t)n_sm * per_sm) ctas = (int64_t)n_sm * per_sm;   // persistent grid: resident CTAs x SMs
     if (ctas < 1) ctas = 1;
-    cossim_candidates_kernel<NW, AccT><<<(unsigned)ctas, NW * 32, smem, st>>>(
-        a_indptr, a_len, a_indices, a_val32, row_begin, row_end, perm_a, n_right, (const int2 *)bucket_dir,
-        (const uint32_t *)bucket_maxw, (const uint32_t *)postings, perm_b, (int)sg_num_tiles_padded(n_right, tile_w),
-        tile_w, T, tiles_per_group,
-        a_scale, thr_c, thr_row, xp_norm, tile_bound, diag_rank, diag_rank ? group_items : nullptr, cand_row, cand_col,
-        cand_partial, (unsigned long long)cand_cap, cand_count, row_queue);
+#define SG_KARGS                                                                                                    \
+    a_indptr, a_len, a_indices, a_val32, row_begin, row_end, perm_a, n_right, (const int2 *)bucket_dir,               \
+        (const uint32_t *)bucket_maxw, (const uint32_t *)postings, perm_b, (int)sg_num_tiles_padded(n_right, tile_w), \
+        tile_w, T, tiles_per_group, a_scale, thr_c, thr_row, xp_norm, tile_bound, diag_rank,                         \
+        diag_rank ? group_items : nullptr, cand_row, cand_col, cand_partial, (unsigned long long)cand_cap, cand_count, \
+        row_queue
+    if constexpr (FLOOR)
+        cossim_candidates_floor_kernel<NW, AccT><<<(unsigned)ctas, NW * 32, smem, st>>>(SG_KARGS, fa);
+    else
+        cossim_candidates_kernel<NW, AccT><<<(unsigned)ctas, NW * 32, smem, st>>>(SG_KARGS);
+#undef SG_KARGS
     SG_LAUNCH_CHECK();
     return SG_OK;
 }
 
-extern "C" {
-
-int sg_cossim_candidates(const int64_t *a_indptr, const int32_t *a_len, const int32_t *a_indices,
-                         const float *a_val32, int64_t row_begin, int64_t row_end, const int32_t *perm_a,
-                         int64_t n_right, int64_t n_cols, const void *bucket_dir, const void *bucket_maxw,
-                         const void *postings, const int32_t *perm_b, int tile_w, int acc_dtype, float a_scale,
-                         float cand_threshold,
-                         const float *cand_threshold_row, const float *pruned_norm_row, const float *tile_bound,
-                         int64_t tiles_per_group, const int32_t *diag_rank, unsigned long long *group_items,
-                         int32_t *cand_row, int32_t *cand_col, float *cand_partial, int64_t cand_cap,
-                         unsigned long long *cand_count, unsigned long long *row_queue, int warps_per_cta,
-                         void *stream_) {
+// fa == NULL: cossim_candidates_kernel; otherwise the floor variant
+static int cossim_candidates(const int64_t *a_indptr, const int32_t *a_len, const int32_t *a_indices,
+                             const float *a_val32, int64_t row_begin, int64_t row_end, const int32_t *perm_a,
+                             int64_t n_right, int64_t n_cols, const void *bucket_dir, const void *bucket_maxw,
+                             const void *postings, const int32_t *perm_b, int tile_w, int acc_dtype, float a_scale,
+                             float cand_threshold,
+                             const float *cand_threshold_row, const float *pruned_norm_row, const float *tile_bound,
+                             int64_t tiles_per_group, const int32_t *diag_rank, unsigned long long *group_items,
+                             int32_t *cand_row, int32_t *cand_col, float *cand_partial, int64_t cand_cap,
+                             unsigned long long *cand_count, unsigned long long *row_queue, int warps_per_cta,
+                             void *stream_, const FloorArgs *fa) {
     cudaStream_t st = (cudaStream_t)stream_;
     if (row_end <= row_begin || n_right <= 0) return SG_OK;
     if (acc_dtype != SG_ACC_F32 && acc_dtype != SG_ACC_U16)
@@ -976,10 +1121,17 @@ int sg_cossim_candidates(const int64_t *a_indptr, const int32_t *a_len, const in
     a_indptr, a_len, a_indices, a_val32, row_begin, row_end, perm_a, n_right, n_cols, bucket_dir, bucket_maxw, \
         postings, perm_b, tile_w, tiles_per_group, a_scale, cand_threshold, cand_threshold_row, pruned_norm_row,      \
         tile_bound, diag_rank, group_items, cand_row, cand_col, cand_partial, cand_cap, cand_count, row_queue, n_sm, st
+    if (fa) {
+        // the floor variant is built for the default 8 warps only
+        if (warps_per_cta != 8) return fail(SG_ERR_INVALID, "the top-n floor variant runs with 8 warps per CTA");
+        return acc_dtype == SG_ACC_U16 ? launch_candidates<8, uint16_t, true>(SG_ARGS, *fa)
+                                       : launch_candidates<8, float, true>(SG_ARGS, *fa);
+    }
+    const FloorArgs none{};
 #define SG_CASE(NW)                                                                                          \
     case NW:                                                                                                 \
-        return acc_dtype == SG_ACC_U16 ? launch_candidates<NW, uint16_t>(SG_ARGS)                           \
-                                       : launch_candidates<NW, float>(SG_ARGS);
+        return acc_dtype == SG_ACC_U16 ? launch_candidates<NW, uint16_t, false>(SG_ARGS, none)              \
+                                       : launch_candidates<NW, float, false>(SG_ARGS, none);
     switch (warps_per_cta) {
         SG_CASE(4)
         SG_CASE(8)
@@ -992,11 +1144,56 @@ int sg_cossim_candidates(const int64_t *a_indptr, const int32_t *a_len, const in
 #undef SG_ARGS
 }
 
-int sg_rescore(int64_t n_cand, const int32_t *cand_row, const int32_t *cand_col, const int64_t *a_indptr,
-               const int32_t *a_indices, const void *a_val, const int64_t *b_indptr, const int32_t *b_indices,
-               const void *b_val, int dtype, double *score_out, double keep_threshold, int32_t *keep_row,
-               int32_t *keep_col, unsigned long long *keep_count, unsigned long long *mirror_count,
-               int32_t *row_cnt, int64_t row_begin, void *stream_) {
+extern "C" {
+
+int sg_cossim_candidates(const int64_t *a_indptr, const int32_t *a_len, const int32_t *a_indices,
+                         const float *a_val32, int64_t row_begin, int64_t row_end, const int32_t *perm_a,
+                         int64_t n_right, int64_t n_cols, const void *bucket_dir, const void *bucket_maxw,
+                         const void *postings, const int32_t *perm_b, int tile_w, int acc_dtype, float a_scale,
+                         float cand_threshold,
+                         const float *cand_threshold_row, const float *pruned_norm_row, const float *tile_bound,
+                         int64_t tiles_per_group, const int32_t *diag_rank, unsigned long long *group_items,
+                         int32_t *cand_row, int32_t *cand_col, float *cand_partial, int64_t cand_cap,
+                         unsigned long long *cand_count, unsigned long long *row_queue, int warps_per_cta,
+                         void *stream_) {
+    return cossim_candidates(a_indptr, a_len, a_indices, a_val32, row_begin, row_end, perm_a, n_right, n_cols,
+                             bucket_dir, bucket_maxw, postings, perm_b, tile_w, acc_dtype, a_scale, cand_threshold,
+                             cand_threshold_row, pruned_norm_row, tile_bound, tiles_per_group, diag_rank, group_items,
+                             cand_row, cand_col, cand_partial, cand_cap, cand_count, row_queue, warps_per_cta, stream_,
+                             nullptr);
+}
+
+int sg_cossim_candidates_floor(const int64_t *a_indptr, const int32_t *a_len, const int32_t *a_indices,
+                               const float *a_val32, int64_t row_begin, int64_t row_end, const int32_t *perm_a,
+                               int64_t n_right, int64_t n_cols, const void *bucket_dir, const void *bucket_maxw,
+                               const void *postings, const int32_t *perm_b, int tile_w, int acc_dtype, float a_scale,
+                               float cand_threshold, const float *cand_threshold_row, const float *pruned_norm_row,
+                               const float *tile_bound, int64_t tiles_per_group, int32_t *cand_row,
+                               int32_t *cand_col, float *cand_partial, int64_t cand_cap,
+                               unsigned long long *cand_count, unsigned long long *row_queue, int warps_per_cta,
+                               float *row_floor, int top_n, float floor_margin, float floor_margin_per_feature,
+                               const int32_t *self_rank, int seed, void *stream_) {
+    if (!row_floor) return fail(SG_ERR_INVALID, "row_floor is required");
+    if (top_n < 1 || top_n > 32) return fail(SG_ERR_INVALID, "the top-n floor supports 1 <= top_n <= 32, got %d", top_n);
+    if (!(floor_margin >= 0.f) || !(floor_margin_per_feature >= 0.f))
+        return fail(SG_ERR_INVALID, "floor margins must be >= 0");
+    if (seed && !self_rank) return fail(SG_ERR_INVALID, "seed needs self_rank");
+    if (self_rank && !perm_a) return fail(SG_ERR_INVALID, "self_rank needs perm_a");
+    const FloorArgs fa{row_floor, self_rank, seed ? 1 : 0, top_n, floor_margin, floor_margin_per_feature};
+    return cossim_candidates(a_indptr, a_len, a_indices, a_val32, row_begin, row_end, perm_a, n_right, n_cols,
+                             bucket_dir, bucket_maxw, postings, perm_b, tile_w, acc_dtype, a_scale, cand_threshold,
+                             cand_threshold_row, pruned_norm_row, tile_bound, tiles_per_group, nullptr, nullptr,
+                             cand_row, cand_col, cand_partial, cand_cap, cand_count, row_queue, warps_per_cta, stream_,
+                             &fa);
+}
+
+}  // extern "C"
+
+static int rescore(int64_t n_cand, const int32_t *cand_row, const int32_t *cand_col, const int64_t *a_indptr,
+                   const int32_t *a_indices, const void *a_val, const int64_t *b_indptr, const int32_t *b_indices,
+                   const void *b_val, int dtype, double *score_out, double keep_threshold, int32_t *keep_row,
+                   int32_t *keep_col, unsigned long long *keep_count, unsigned long long *mirror_count,
+                   int32_t *row_cnt, int64_t row_begin, void *stream_, const RescoreFloor &rf) {
     cudaStream_t st = (cudaStream_t)stream_;
     if (n_cand <= 0) return SG_OK;
     if (keep_count && (!keep_row || !keep_col)) return fail(SG_ERR_INVALID, "keep_count needs keep_row and keep_col");
@@ -1007,7 +1204,8 @@ int sg_rescore(int64_t n_cand, const int32_t *cand_row, const int32_t *cand_col,
 #define SG_RESCORE(T, VEC)                                                                                        \
     rescore_kernel<T, VEC><<<grid, 256, 0, st>>>(n_cand, cand_row, cand_col, a_indptr, a_indices, (const T *)a_val, \
                                                  b_indptr, b_indices, (const T *)b_val, score_out, keep_threshold,  \
-                                                 keep_row, keep_col, keep_count, mirror_count, row_cnt, row_begin)
+                                                 keep_row, keep_col, keep_count, mirror_count, row_cnt, row_begin, rf)
+    if (rf.floor && !keep_count) return fail(SG_ERR_INVALID, "row_floor needs keep_count");
     if (dtype == SG_DTYPE_F64) {
         if (vec) SG_RESCORE(double, 1);
         else SG_RESCORE(double, 0);
@@ -1022,13 +1220,14 @@ int sg_rescore(int64_t n_cand, const int32_t *cand_row, const int32_t *cand_col,
     return SG_OK;
 }
 
-int sg_rescore_refined(int64_t n_cand, const int32_t *cand_row, const int32_t *cand_col, const float *cand_partial,
-                       const void *left_group_norms, const void *right_group_norms, const float *row_threshold,
-                       const int64_t *a_indptr, const int32_t *a_indices, const void *a_val,
-                       const int64_t *b_indptr, const int32_t *b_indices, const void *b_val, int dtype,
-                       double *score_out, double keep_threshold, int32_t *keep_row, int32_t *keep_col,
-                       unsigned long long *keep_count, unsigned long long *refined_count,
-                       unsigned long long *mirror_count, int32_t *row_cnt, int64_t row_begin, void *stream_) {
+static int rescore_refined(int64_t n_cand, const int32_t *cand_row, const int32_t *cand_col, const float *cand_partial,
+                           const void *left_group_norms, const void *right_group_norms, const float *row_threshold,
+                           const int64_t *a_indptr, const int32_t *a_indices, const void *a_val,
+                           const int64_t *b_indptr, const int32_t *b_indices, const void *b_val, int dtype,
+                           double *score_out, double keep_threshold, int32_t *keep_row, int32_t *keep_col,
+                           unsigned long long *keep_count, unsigned long long *refined_count,
+                           unsigned long long *mirror_count, int32_t *row_cnt, int64_t row_begin, void *stream_,
+                           const RescoreFloor &rf) {
     cudaStream_t st = (cudaStream_t)stream_;
     if (n_cand <= 0) return SG_OK;
     if (!keep_count || !keep_row || !keep_col) return fail(SG_ERR_INVALID, "keep_count, keep_row and keep_col are required");
@@ -1042,7 +1241,8 @@ int sg_rescore_refined(int64_t n_cand, const int32_t *cand_row, const int32_t *c
     rescore_refined_kernel<T, VEC><<<grid, 256, 0, st>>>(                                                           \
         n_cand, cand_row, cand_col, cand_partial, (const uint4 *)left_group_norms, (const uint4 *)right_group_norms, \
         row_threshold, a_indptr, a_indices, (const T *)a_val, b_indptr, b_indices, (const T *)b_val, score_out,      \
-        keep_threshold, keep_row, keep_col, keep_count, refined_count, mirror_count, row_cnt, row_begin)
+        keep_threshold, keep_row, keep_col, keep_count, refined_count, mirror_count, row_cnt, row_begin, rf)
+    if (rf.floor && !rf.row_len) return fail(SG_ERR_INVALID, "row_floor needs row_len");
     if (dtype == SG_DTYPE_F64) {
         if (vec) SG_RESCORE(double, 1);
         else SG_RESCORE(double, 0);
@@ -1055,6 +1255,59 @@ int sg_rescore_refined(int64_t n_cand, const int32_t *cand_row, const int32_t *c
 #undef SG_RESCORE
     SG_LAUNCH_CHECK();
     return SG_OK;
+}
+
+extern "C" {
+
+int sg_rescore(int64_t n_cand, const int32_t *cand_row, const int32_t *cand_col, const int64_t *a_indptr,
+               const int32_t *a_indices, const void *a_val, const int64_t *b_indptr, const int32_t *b_indices,
+               const void *b_val, int dtype, double *score_out, double keep_threshold, int32_t *keep_row,
+               int32_t *keep_col, unsigned long long *keep_count, unsigned long long *mirror_count,
+               int32_t *row_cnt, int64_t row_begin, void *stream_) {
+    return rescore(n_cand, cand_row, cand_col, a_indptr, a_indices, a_val, b_indptr, b_indices, b_val, dtype,
+                   score_out, keep_threshold, keep_row, keep_col, keep_count, mirror_count, row_cnt, row_begin, stream_,
+                   RescoreFloor{});
+}
+
+int sg_rescore_floor(int64_t n_cand, const int32_t *cand_row, const int32_t *cand_col, const int64_t *a_indptr,
+                     const int32_t *a_indices, const void *a_val, const int64_t *b_indptr, const int32_t *b_indices,
+                     const void *b_val, int dtype, double *score_out, double keep_threshold, int32_t *keep_row,
+                     int32_t *keep_col, unsigned long long *keep_count, int32_t *row_cnt, int64_t row_begin,
+                     const float *row_floor, unsigned long long *floor_dropped, void *stream_) {
+    if (!row_floor) return fail(SG_ERR_INVALID, "row_floor is required");
+    return rescore(n_cand, cand_row, cand_col, a_indptr, a_indices, a_val, b_indptr, b_indices, b_val, dtype,
+                   score_out, keep_threshold, keep_row, keep_col, keep_count, nullptr, row_cnt, row_begin, stream_,
+                   RescoreFloor{row_floor, nullptr, 0.f, 0.f, floor_dropped});
+}
+
+int sg_rescore_refined(int64_t n_cand, const int32_t *cand_row, const int32_t *cand_col, const float *cand_partial,
+                       const void *left_group_norms, const void *right_group_norms, const float *row_threshold,
+                       const int64_t *a_indptr, const int32_t *a_indices, const void *a_val,
+                       const int64_t *b_indptr, const int32_t *b_indices, const void *b_val, int dtype,
+                       double *score_out, double keep_threshold, int32_t *keep_row, int32_t *keep_col,
+                       unsigned long long *keep_count, unsigned long long *refined_count,
+                       unsigned long long *mirror_count, int32_t *row_cnt, int64_t row_begin, void *stream_) {
+    return rescore_refined(n_cand, cand_row, cand_col, cand_partial, left_group_norms, right_group_norms,
+                           row_threshold, a_indptr, a_indices, a_val, b_indptr, b_indices, b_val, dtype, score_out,
+                           keep_threshold, keep_row, keep_col, keep_count, refined_count, mirror_count, row_cnt,
+                           row_begin, stream_, RescoreFloor{});
+}
+
+int sg_rescore_refined_floor(int64_t n_cand, const int32_t *cand_row, const int32_t *cand_col,
+                             const float *cand_partial, const void *left_group_norms, const void *right_group_norms,
+                             const float *row_threshold, const int64_t *a_indptr, const int32_t *a_indices,
+                             const void *a_val, const int64_t *b_indptr, const int32_t *b_indices, const void *b_val,
+                             int dtype, double *score_out, double keep_threshold, int32_t *keep_row,
+                             int32_t *keep_col, unsigned long long *keep_count, unsigned long long *refined_count,
+                             int32_t *row_cnt, int64_t row_begin, const float *row_floor, const int32_t *row_len,
+                             float floor_margin, float floor_margin_per_feature, unsigned long long *floor_dropped,
+                             void *stream_) {
+    if (!row_floor) return fail(SG_ERR_INVALID, "row_floor is required");
+    return rescore_refined(n_cand, cand_row, cand_col, cand_partial, left_group_norms, right_group_norms,
+                           row_threshold, a_indptr, a_indices, a_val, b_indptr, b_indices, b_val, dtype, score_out,
+                           keep_threshold, keep_row, keep_col, keep_count, refined_count, nullptr, row_cnt, row_begin,
+                           stream_, RescoreFloor{row_floor, row_len, floor_margin, floor_margin_per_feature,
+                                                 floor_dropped});
 }
 
 int sg_rowwise_dot(int64_t n_rows, const int64_t *a_indptr, const int32_t *a_indices, const void *a_val,

@@ -52,6 +52,7 @@ __global__ void prune_rows_kernel(int64_t row_begin, int64_t n_rows, const int64
                                   const int32_t *__restrict__ df_right, const int8_t *__restrict__ prunable,
                                   float right_norm, float budget,
                                   float threshold, float margin, float margin_per_feature,
+                                  const float *__restrict__ row_floor, float frac,
                                   int32_t *__restrict__ out_idx, float *__restrict__ out_val,
                                   int32_t *__restrict__ out_len, float *__restrict__ out_thr,
                                   float *__restrict__ out_xp, __half *__restrict__ out_xg) {
@@ -61,6 +62,10 @@ __global__ void prune_rows_kernel(int64_t row_begin, int64_t n_rows, const int64
     const int64_t row = row_begin + r;
     const int64_t p0 = indptr[row];
     const int nf = (int)(indptr[row + 1] - p0);
+    if (row_floor) {        // per-row threshold: score > max(threshold, floor - FLOOR_EPS) covers score >= floor
+        threshold = fmaxf(threshold, row_floor[row] - FLOOR_EPS);
+        budget = fmaxf(frac * (threshold - margin), 0.f);
+    }
     // |x_P| <= budget / max|y|
     const float lim = right_norm > 0.f ? budget / right_norm : 0.f;
     const float lim2 = lim * lim;
@@ -225,8 +230,29 @@ int sg_prune_rows(int64_t row_begin, int64_t row_end, const int64_t *indptr, con
     if (out_group_norms && !prunable) return fail(SG_ERR_INVALID, "group norms need the heavy-feature ranks");
     prune_rows_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(row_begin, n, indptr, indices, val32, df_right,
                                                               prunable, right_norm, budget, threshold, margin,
-                                                              margin_per_feature, out_indices, out_val32, out_len,
-                                                              out_threshold, out_pruned_norm,
+                                                              margin_per_feature, nullptr, 0.f, out_indices,
+                                                              out_val32, out_len, out_threshold, out_pruned_norm,
+                                                              (__half *)out_group_norms);
+    SG_LAUNCH_CHECK();
+    return SG_OK;
+}
+
+int sg_prune_rows_floor(int64_t row_begin, int64_t row_end, const int64_t *indptr, const int32_t *indices,
+                        const float *val32, const int32_t *df_right, const int8_t *prunable, float right_norm,
+                        float frac, float threshold, const float *row_floor, float margin, float margin_per_feature,
+                        int32_t *out_indices, float *out_val32, int32_t *out_len, float *out_threshold,
+                        float *out_pruned_norm, void *out_group_norms, void *stream_) {
+    cudaStream_t st = (cudaStream_t)stream_;
+    const int64_t n = row_end - row_begin;
+    if (n <= 0) return SG_OK;
+    if (!row_floor) return fail(SG_ERR_INVALID, "row_floor is required");
+    if (!(frac >= 0.f) || !(frac < 1.f) || !(right_norm >= 0.f))
+        return fail(SG_ERR_INVALID, "frac must lie in [0, 1) and right_norm be >= 0");
+    if (out_group_norms && !prunable) return fail(SG_ERR_INVALID, "group norms need the heavy-feature ranks");
+    prune_rows_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(row_begin, n, indptr, indices, val32, df_right,
+                                                              prunable, right_norm, 0.f, threshold, margin,
+                                                              margin_per_feature, row_floor, frac, out_indices,
+                                                              out_val32, out_len, out_threshold, out_pruned_norm,
                                                               (__half *)out_group_norms);
     SG_LAUNCH_CHECK();
     return SG_OK;
