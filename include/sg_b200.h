@@ -267,9 +267,14 @@ int sg_cossim_candidates(const int64_t *a_indptr /*[dev]*/, const int32_t *a_len
  * keeps the best 32 values (partial - E_r, rounded down) of the pairs it reported and, once it holds top_n of them,
  * raises row_floor[row] to the top_n-th with atomicMax; the floor is read again at every batch of 64 column tiles.
  * Self-match (`self_rank` [dev] per row id: the row's position in the common processing order, perm_a the same
- * order): `seed` = 1 walks only the column-tile group holding the row, starting at the 64-tile batch that holds it;
- * seed = 0 walks every other group.  self_rank = NULL: every group (two matrices).
+ * order): `flags` & SG_FLOOR_SEED walks only the column-tile group holding the row, starting at the 64-tile batch that
+ * holds it; without it every other group.  self_rank = NULL: every group (two matrices).
+ * `flags` & SG_FLOOR_LONG_ROWS (acc_dtype SG_ACC_F32 only): rows with more than 32 kept features are bounded by the
+ * block-max test over all their features too, instead of walking every tile (the no-threshold mode of the top-n
+ * product, where long rows keep all their features).
  */
+#define SG_FLOOR_SEED 1
+#define SG_FLOOR_LONG_ROWS 2
 int sg_cossim_candidates_floor(const int64_t *a_indptr /*[dev]*/, const int32_t *a_len /*[dev] or NULL*/,
                                const int32_t *a_indices /*[dev]*/, const float *a_val32 /*[dev]*/,
                                int64_t row_begin, int64_t row_end, const int32_t *perm_a /*[dev] or NULL*/,
@@ -284,7 +289,7 @@ int sg_cossim_candidates_floor(const int64_t *a_indptr /*[dev]*/, const int32_t 
                                unsigned long long *cand_count /*[dev] 1*/, unsigned long long *row_queue /*[dev] 1*/,
                                int warps_per_cta, float *row_floor /*[dev] per left row id*/, int top_n,
                                float floor_margin, float floor_margin_per_feature,
-                               const int32_t *self_rank /*[dev] per row id, or NULL*/, int seed, void *stream);
+                               const int32_t *self_rank /*[dev] per row id, or NULL*/, int flags, void *stream);
 
 /* ------------------------------------------------------------------------- *
  * K2, tile-centric form (csrc/sg_tiles.cu) — the default for L2-normalised non-negative matrices (K1 output).
@@ -481,6 +486,12 @@ int sg_row_order(int64_t row_begin, int64_t row_end, const int64_t *indptr, cons
                  const int8_t *hrank, const float *row_norm /*[dev] or NULL*/, float norm_scale,
                  int32_t *perm /*[dev]*/, int32_t *rank /*[dev] or NULL*/, void *ws,
                  size_t ws_bytes, void *stream);
+/* keys[i] = the 64-bit key sg_row_order sorts row row_begin + i by, computed by the same kernel from the same
+ * arguments (unsigned order).  A row of another matrix, keyed with the right matrix's hrank and norm scale, finds its
+ * position in the right matrix's sorted order by a binary search over the right keys in that order. */
+int sg_row_keys(int64_t row_begin, int64_t row_end, const int64_t *indptr, const int32_t *indices,
+                const int8_t *hrank, const float *row_norm /*[dev] or NULL*/, float norm_scale,
+                uint64_t *keys /*[dev] row_end - row_begin*/, void *stream);
 
 /* ------------------------------------------------------------------------- *
  * K4 — self-match post-processing.

@@ -488,7 +488,9 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
     `floor` (None = SG_B200_TOPN_FLOOR, default "auto"; True; False): the top-n floor of DESIGN.md §4, which bounds
     the candidates of low thresholds by each row's top_n-th best score.  "auto" takes it only where the usual path
     would not fit: top_n <= 32, threshold < 0.5, at least FLOOR_MIN_ROWS rows, and a sampled candidate count whose
-    24 bytes each exceed a quarter of device memory.  True needs top_n <= 32, threshold > 0 and non-negative operands.
+    24 bytes each exceed a quarter of device memory.  True needs top_n <= 32 and non-negative operands.  A threshold
+    <= 0 (no threshold: every pair with a positive score counts) starts the floors from the exact scores of each
+    row's neighbours in the processing order (topn_floor_init).
     """
     t = require_cuda()
     L = _lib.load()
@@ -510,12 +512,12 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
 
     if floor not in (None, "auto", True, False):
         raise ValueError("floor must be None, 'auto', True or False, got %r" % (floor,))
-    floor_ok = top_n <= 32 and float(threshold) > 0.0 and A.nonneg and B.nonneg
+    floor_ok = top_n <= 32 and A.nonneg and B.nonneg
     if floor is None:       # the environment knob forces the floor only where it applies
         floor = TOPN_FLOOR if (TOPN_FLOOR is not True or floor_ok) else False
     if floor is True:
         if not floor_ok:
-            raise ValueError("the top-n floor needs top_n <= 32, min_similarity > 0 and non-negative matrices")
+            raise ValueError("the top-n floor needs top_n <= 32 and non-negative matrices")
         if (kernel or "row").lower() != "row":
             raise ValueError("the top-n floor runs on the row kernel only")
     if floor is True or (floor == "auto" and floor_ok and float(threshold) < 0.5 and n_rows >= FLOOR_MIN_ROWS):
@@ -822,6 +824,88 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
                         shape, stats)
 
 
+FLOOR_INIT_WINDOW = 64      # right rows around each left row's position whose exact scores start its floor
+
+
+def row_keys(M, hrank, row_begin=0, row_end=None, row_norm=None, norm_scale=1.0):
+    """int64 sort key of rows [row_begin,row_end) of M: the 64-bit key sg_row_order sorts by (sg_row_keys) with the
+    top bit flipped, so that signed order is the kernel's unsigned order."""
+    t = require_cuda()
+    L = _lib.load()
+    row_end = M.shape[0] if row_end is None else row_end
+    keys = _empty(row_end - row_begin, t.int64, M.device)
+    _lib.check(L.sg_row_keys(row_begin, row_end, _ptr(M.d_indptr), _ptr(M.d_indices), _ptr(hrank), _ptr(row_norm),
+                             float(norm_scale), _ptr(keys), _stream()))
+    LAUNCH_COUNTS["order"] += 1
+    return keys ^ t.iinfo(t.int64).min
+
+
+def topn_floor_init(A, B, top_n, threshold, row_begin=0, row_end=None):
+    """Initial top-n floors of rows [row_begin,row_end) of A against B (DESIGN.md §4): fp32 [A.shape[0]], zero
+    outside the range.
+
+    Both sides sort by the same key (sg_row_order), so similar rows sit next to each other.  Each left row takes the
+    FLOOR_INIT_WINDOW right rows around its position in the right matrix's order (a self-match: the row's own rank;
+    two matrices: the insertion point of its key among the sorted right keys); the window is shifted, not clamped, at
+    the ends, so its columns are distinct.  sg_rescore scores the pairs exactly and keeps those above
+    max(threshold, 0); the floor is the top_n-th best of them (sg_topn_select_rows), 0 for a row with fewer, written
+    in fp32 rounded down.  It is the top_n-th best exact score of top_n distinct real pairs above the threshold, so it
+    never exceeds the row's exact top_n-th best."""
+    t = require_cuda()
+    L = _lib.load()
+    row_end = A.shape[0] if row_end is None else int(row_end)
+    n_rows, n_right = row_end - row_begin, B.shape[0]
+    dev = A.device
+    floor = t.zeros(A.shape[0], dtype=t.float32, device=dev)
+    K = min(FLOOR_INIT_WINDOW, n_right)
+    top_n = int(min(int(top_n), n_right))
+    if n_rows <= 0 or K == 0 or top_n <= 0:
+        return floor
+    hrank, perm_b, rank_b = right_order(B)
+    if A is B:
+        pos = rank_b[row_begin:row_end].long()
+    else:
+        scale = 1.0 / max(B.norm_bound, 1e-30)        # the norm scale of right_order(B)
+        keys_b = row_keys(B, hrank, row_norm=B._heavy_norm, norm_scale=scale)[perm_b.long()]
+        keys_a = row_keys(A, hrank, row_begin, row_end, heavy_norms(A, hrank, row_begin, row_end), scale)
+        pos = t.searchsorted(keys_b, keys_a)
+    start = (pos - K // 2).clamp(0, n_right - K)
+    cand_col = perm_b[(start[:, None] + t.arange(K, device=dev)).reshape(-1)].contiguous()
+    cand_row = t.arange(row_begin, row_end, dtype=t.int32, device=dev).repeat_interleave(K)
+    n = n_rows * K
+    score = _empty(n, t.float64, dev)
+    keep_row, keep_col = _empty(n, t.int32, dev), _empty(n, t.int32, dev)
+    count = t.zeros(1, dtype=t.int64, device=dev)
+    row_cnt = t.zeros(n_rows + 1, dtype=t.int32, device=dev)
+    dt = _lib.SG_DTYPE_F32 if A.dtype == np.float32 else _lib.SG_DTYPE_F64
+    _lib.check(L.sg_rescore(n, _ptr(cand_row), _ptr(cand_col), _ptr(A.d_indptr), _ptr(A.d_indices), _ptr(A.d_val),
+                            _ptr(B.d_indptr), _ptr(B.d_indices), _ptr(B.d_val), dt, _ptr(score),
+                            max(float(threshold), 0.0), _ptr(keep_row), _ptr(keep_col), _ptr(count), None,
+                            _ptr(row_cnt), row_begin, _stream()))
+    LAUNCH_COUNTS["rescore"] += 1
+    del cand_row, cand_col
+    n_keep = int(count.item())
+    if n_keep == 0:
+        return floor
+    out_indptr = _empty(n_rows + 1, t.int64, dev)
+    out_row, out_col, out_score = _empty(n_keep, t.int32, dev), _empty(n_keep, t.int32, dev), _empty(n_keep, t.float64, dev)
+    tail = t.zeros(2, dtype=t.int64, device=dev)
+    ws_bytes = int(L.sg_topn_select_rows_workspace_bytes(n_keep, n_rows))
+    ws = _empty(ws_bytes, t.uint8, dev)
+    _lib.check(L.sg_topn_select_rows(n_keep, _ptr(keep_row), _ptr(keep_col), _ptr(score), row_begin, n_rows, top_n,
+                                     _ptr(row_cnt), _ptr(out_indptr), _ptr(out_row), _ptr(out_col), _ptr(out_score),
+                                     ctypes.c_void_p(tail.data_ptr()), ctypes.c_void_p(tail.data_ptr() + 8), _ptr(ws),
+                                     ws_bytes, _stream()))
+    LAUNCH_COUNTS["select"] += 6
+    # rows are written score-descending: the last of a full row is its top_n-th best
+    full = (out_indptr[1:] - out_indptr[:-1]) == top_n
+    kth = t.where(full, out_score[(out_indptr[1:] - 1).clamp(0, n_keep - 1)], t.zeros((), dtype=t.float64, device=dev))
+    f32 = kth.float()
+    f32 = t.where(f32.double() > kth, t.nextafter(f32, t.full_like(f32, -float("inf"))), f32)     # rounded down
+    floor[row_begin:row_end] = f32.clamp_min(0.0)
+    return floor
+
+
 def _cossim_topn_floor(A, B, top_n, threshold, row_begin, row_end, tile_w, stats, prune, acc, decide):
     """cossim_topn with the top-n floor (DESIGN.md §4): row kernel, full product (no triangle), 8 warps per CTA.
 
@@ -830,7 +914,11 @@ def _cossim_topn_floor(A, B, top_n, threshold, row_begin, row_end, tile_w, stats
     identical names set high floors at once), prunes the left rows again for max(threshold, floor), then walks the
     other groups.  The re-score keeps only pairs at or above the floor, which changes no output.  With `decide` the
     floor is taken only if the sampled candidate count of the usual path needs more than a quarter of device memory;
-    otherwise None is returned and the caller runs the usual path."""
+    otherwise None is returned and the caller runs the usual path.
+
+    threshold <= 0 (no threshold): the floors start from topn_floor_init, the left rows are pruned against them
+    before the first launch, and the candidates kernel bounds rows of more than 32 kept features by the block-max test
+    as well (SG_FLOOR_LONG_ROWS); the accumulator is fp32."""
     t = require_cuda()
     L = _lib.load()
     n_left, n_right = A.shape[0], B.shape[0]
@@ -847,9 +935,14 @@ def _cossim_topn_floor(A, B, top_n, threshold, row_begin, row_end, tile_w, stats
         acc = "f32"
     acc_code = _lib.SG_ACC_U16 if acc == "u16" else _lib.SG_ACC_F32
     margin_pf = U16_MARGIN_PER_FEATURE if acc == "u16" else 0.0
+    no_threshold = threshold <= 0.0
     level = PRUNE_FRAC if prune is None else float(prune)
+    # pruning level of the re-pruning against the floors; without a threshold the floors are all there is to prune for
+    floor_level = level
     if thr_c <= 0.0:
         level = 0.0
+        if not no_threshold:
+            floor_level = 0.0
     warps = 8                                   # the floor variant of the candidates kernel is built for 8 warps
     tile_w, _ = pick_tile(n_right, tile_w, warps, 2 if acc == "u16" else 4, n_left=n_rows)
     while (-(-n_right // tile_w)) * (B.shape[1] + 1) > MAX_BUCKETS and tile_w < 32768:
@@ -877,11 +970,12 @@ def _cossim_topn_floor(A, B, top_n, threshold, row_begin, row_end, tile_w, stats
         sample = perm_a[:n_rows:stride].contiguous()
 
     def pruned(row_floor=None):
-        if level <= 0.0 and margin_pf <= 0.0:
+        lv = level if row_floor is None else floor_level
+        if lv <= 0.0 and margin_pf <= 0.0:
             return (A.d_indices, A.d_val32, None, None, None, None)
         if row_floor is None:
-            return prune_left(A, B, hrank, row_begin, row_end, threshold, margin, margin_pf, level)
-        return prune_left_floor(A, B, hrank, row_begin, row_end, threshold, margin, margin_pf, level, row_floor)
+            return prune_left(A, B, hrank, row_begin, row_end, threshold, margin, margin_pf, lv)
+        return prune_left_floor(A, B, hrank, row_begin, row_end, threshold, margin, margin_pf, lv, row_floor)
 
     arrays = pruned()
     mark(stats, "right_side")
@@ -902,7 +996,16 @@ def _cossim_topn_floor(A, B, top_n, threshold, row_begin, row_end, tile_w, stats
             stats["n_candidates_estimate_usual"] = est_usual
         if est_usual * 24 <= total_mem // 4:
             return None
-    floor_buf = t.zeros(n_left, dtype=t.float32, device=dev)
+    n_init_positive = None
+    if no_threshold:
+        # without a threshold every touched column is a candidate until a floor rises: start from proven floors
+        floor_buf = topn_floor_init(A, B, top_n, threshold, row_begin, row_end)
+        n_init_positive = int((floor_buf[row_begin:row_end] > 0).sum().item())
+        arrays = pruned(floor_buf)
+        mark(stats, "floor_init")
+    else:
+        floor_buf = t.zeros(n_left, dtype=t.float32, device=dev)
+    flags = _lib.SG_FLOOR_LONG_ROWS if no_threshold else 0
 
     def launch(perm, n, arrs, row_buf, col_buf, part_buf, capacity, seed):
         l_idx, l_val, l_len, l_thr, l_xp, _ = arrs
@@ -912,7 +1015,7 @@ def _cossim_topn_floor(A, B, top_n, threshold, row_begin, row_end, tile_w, stats
             A.shape[1], _ptr(bucket_dir), _ptr(bucket_maxw), _ptr(post), _ptr(perm_b), tile_w, acc_code,
             max(B.norm_bound, 1.0), thr_c, _ptr(l_thr), _ptr(l_xp), _ptr(tile_bound), tiles_per_group, _ptr(row_buf),
             _ptr(col_buf), _ptr(part_buf), capacity, c_count, c_queue, warps, _ptr(floor_buf), top_n, margin,
-            margin_pf, _ptr(self_rank), 1 if seed else 0, _stream()))
+            margin_pf, _ptr(self_rank), flags | (_lib.SG_FLOOR_SEED if seed else 0), _stream()))
         LAUNCH_COUNTS["candidates"] += 1
         return int(counters[0].item())
 
@@ -1017,7 +1120,15 @@ def _cossim_topn_floor(A, B, top_n, threshold, row_begin, row_end, tile_w, stats
     mark(stats, "rescore")
     if stats is not None:
         stats["topn_floor"] = True
-        stats["prune"], stats["acc"], stats["kernel"] = level, acc, "row"
+        stats["floor_init"] = no_threshold
+        if no_threshold:
+            stats["n_candidates_init"] = n_rows * min(FLOOR_INIT_WINDOW, n_right)     # pairs scored by the init
+            stats["n_floor_init_positive"] = n_init_positive
+            l_len = arrays[2]
+            kept = (l_len[row_begin:row_end] if l_len is not None else
+                    A.d_indptr[row_begin + 1:row_end + 1] - A.d_indptr[row_begin:row_end])
+            stats["n_rows_long"] = int((kept > 32).sum().item())      # bounded by SG_FLOOR_LONG_ROWS
+        stats["prune"], stats["acc"], stats["kernel"] = (floor_level if no_threshold else level), acc, "row"
         stats["n_candidates_estimate"] = est
         stats["n_candidates_seed"], stats["n_candidates_main"] = n_seed, n_main
         stats["n_candidates"] = n_seed + n_main

@@ -23,6 +23,8 @@ SG_SYMM_FIX_DIAGONAL = 1
 SG_SYMM_MIRROR = 2
 SG_ACC_F32 = 0
 SG_ACC_U16 = 1
+SG_FLOOR_SEED = 1
+SG_FLOOR_LONG_ROWS = 2
 
 _i64 = ctypes.c_int64
 _i32 = ctypes.c_int
@@ -76,6 +78,7 @@ SIGNATURES = {
     "sg_order_workspace_bytes": (_sz, [_i64, _i64]),
     "sg_heavy_features": (_i32, [_i64, _i64, _p, _p, _p, _i32, _p, _p, _sz, _p]),
     "sg_row_order": (_i32, [_i64, _i64, _p, _p, _p, _p, _f32, _p, _p, _p, _sz, _p]),
+    "sg_row_keys": (_i32, [_i64, _i64, _p, _p, _p, _p, _f32, _p, _p]),
     "sg_rescore": (_i32, [_i64, _p, _p, _p, _p, _p, _p, _p, _p, _i32, _p, _f64, _p, _p, _p, _p, _p, _i64, _p]),
     "sg_rescore_refined": (_i32, [_i64, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i32, _p, _f64, _p, _p, _p, _p,
                                   _p, _p, _i64, _p]),

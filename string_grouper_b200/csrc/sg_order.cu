@@ -67,7 +67,7 @@ __global__ void order_signature_kernel(int64_t row_begin, int64_t n_rows, const 
             s = ((uint64_t)q << 59) | (s >> 5);
         }
         sig[r] = s;
-        ids[r] = (int32_t)row;
+        if (ids) ids[r] = (int32_t)row;
     }
 }
 
@@ -153,6 +153,19 @@ int sg_row_order(int64_t row_begin, int64_t row_end, const int64_t *indptr, cons
         order_inverse_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, row_begin, perm, rank);
         SG_LAUNCH_CHECK();
     }
+    return SG_OK;
+}
+
+// keys[i] = the key sg_row_order sorts row row_begin + i by (same kernel): rows of another matrix find their place in
+// a sorted order with a binary search over the sorted keys.
+int sg_row_keys(int64_t row_begin, int64_t row_end, const int64_t *indptr, const int32_t *indices,
+                const int8_t *hrank, const float *row_norm, float norm_scale, uint64_t *keys, void *stream_) {
+    cudaStream_t st = (cudaStream_t)stream_;
+    const int64_t n = row_end - row_begin;
+    if (n <= 0) return SG_OK;
+    order_signature_kernel<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(row_begin, n, indptr, indices, hrank, row_norm,
+                                                                   norm_scale, keys, nullptr);
+    SG_LAUNCH_CHECK();
     return SG_OK;
 }
 
