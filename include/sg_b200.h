@@ -71,28 +71,31 @@ int sg_tfidf_count(const uint8_t *bytes /*[dev]*/, const int64_t *offsets /*[dev
                    int32_t *row_nnz /*[dev] n_docs+1*/, void *stream);
 
 /*
- * Phase 2 (sg_tfidf_finalize): exclusive scan of row_nnz -> indptr (int64);
+ * Phase 2 (sg_tfidf_vocab): exclusive scan of row_nnz -> indptr (int64);
  * exclusive scan of (df > 0) over the key table -> rank_table[key] = column id
- * = rank of the n-gram in sorted order (sklearn _sort_features);
- * idf = ln((1+n)/(1+df)) + 1 and x = tf*idf in the matrix dtype; row L2 norm
- * accumulated in double in column order, IEEE sqrt and divide (sklearn
+ * = rank of the n-gram in sorted order (sklearn _sort_features).
+ * `vocab_size` [dev] receives V, `nnz_total` [dev] receives indptr[n_docs].
+ * The host then reads V and df in column order (sg_tfidf_vocab_df) back and
+ * computes idf[V] in the matrix dtype exactly as TfidfTransformer.fit does on
+ * the host (numpy's log: its result is not the device's log).
+ *
+ * Phase 3 (sg_tfidf_values): x = tf*idf[column] in the matrix dtype; row L2
+ * norm accumulated in double in column order, IEEE sqrt and divide (sklearn
  * _inplace_csr_row_normalize_l2); writes indices, values in the matrix dtype
  * (val64 for f64, may be NULL for f32) and an fp32 copy for K2.
- * `vocab_size` [dev] receives V, `nnz_total` [dev] receives indptr[n_docs].
  * The caller sizes indices/val64/val32 with total_bytes entries (an upper
- * bound of nnz), so no host read-back is needed between the two phases.
+ * bound of nnz).
  */
-size_t sg_tfidf_finalize_workspace_bytes(int64_t n_docs, int ngram);
-int sg_tfidf_finalize(const int64_t *offsets /*[dev]*/, int64_t n_docs,
-                      int64_t n_docs_fit /* documents counted in df_table: n_docs, or the global count when the
-                                            corpus is sharded over GPUs and df_table was all-reduced */,
-                      int ngram, int dtype,
-                      const int32_t *df_table /*[dev]*/, int32_t *rank_table /*[dev] slots*/,
-                      const uint32_t *scratch_key, const uint32_t *scratch_tf, int32_t *row_nnz,
-                      int64_t *indptr /*[dev] n_docs+1*/, int32_t *indices /*[dev]*/,
-                      double *val64 /*[dev]*/, float *val32 /*[dev]*/,
-                      int32_t *vocab_size /*[dev] 1*/, int64_t *nnz_total /*[dev] 1*/,
-                      void *ws /*[dev]*/, size_t ws_bytes, void *stream);
+size_t sg_tfidf_vocab_workspace_bytes(int64_t n_docs, int ngram);
+int sg_tfidf_vocab(int64_t n_docs, int ngram, const int32_t *df_table /*[dev]*/, int32_t *rank_table /*[dev] slots*/,
+                   int32_t *row_nnz /*[dev] n_docs+1*/, int64_t *indptr /*[dev] n_docs+1*/,
+                   int32_t *vocab_size /*[dev] 1*/, int64_t *nnz_total /*[dev] 1*/, void *ws /*[dev]*/,
+                   size_t ws_bytes, void *stream);
+int sg_tfidf_values(const int64_t *offsets /*[dev]*/, int64_t n_docs, int dtype,
+                    const void *idf /*[dev] V, matrix dtype*/, const int32_t *rank_table /*[dev]*/,
+                    const uint32_t *scratch_key, const uint32_t *scratch_tf, const int32_t *row_nnz,
+                    const int64_t *indptr /*[dev] n_docs+1*/, int32_t *indices /*[dev]*/,
+                    double *val64 /*[dev]*/, float *val32 /*[dev]*/, void *stream);
 
 /* keys_out[c] = packed n-gram of column c (sorted vocabulary), V entries. */
 int sg_tfidf_vocab_keys(const int32_t *df_table /*[dev]*/, const int32_t *rank_table /*[dev]*/, int ngram,
@@ -112,21 +115,25 @@ int sg_tfidf_vocab_df(const int32_t *df_table /*[dev]*/, const int32_t *rank_tab
  * `offsets` count symbols.  Phase 1 writes, per document, its sorted distinct keys and term counts at the document's
  * offset in scratch_key / scratch_tf and row_nnz[doc]; scratch_clean / scratch_sort serve documents longer than 256
  * symbols.  Phase 2: indptr; ONE radix sort of all (document, key) runs -> vocabulary (vocab_keys[c] = key of column c,
- * df[c]), column ids by a scan; values as sg_tfidf_finalize.  No device-to-host read-back inside either call.
+ * df[c]), column ids by a scan, written to indices (sg_tfidf64_vocab).  The host reads V and df[:V] back and computes
+ * idf[V] (as for sg_tfidf_vocab); sg_tfidf64_values then writes the values as sg_tfidf_values does.  No device-to-host
+ * read-back inside any call.
  * ------------------------------------------------------------------------- */
 int sg_tfidf64_count(const void *symbols /*[dev]*/, int sym_width, const int64_t *offsets /*[dev] n_docs+1*/,
                      int64_t n_docs, int ngram, int bits, const uint8_t *lut /*[dev] 256 or NULL*/,
                      uint32_t *scratch_clean /*[dev] total*/, uint64_t *scratch_sort /*[dev] total*/,
                      uint64_t *scratch_key /*[dev] total*/, uint32_t *scratch_tf /*[dev] total*/,
                      int32_t *row_nnz /*[dev] n_docs+1*/, void *stream);
-size_t sg_tfidf64_finalize_workspace_bytes(int64_t n_docs, int64_t total_symbols);
-int sg_tfidf64_finalize(const int64_t *offsets /*[dev]*/, int64_t n_docs, int64_t n_docs_fit, int64_t total_symbols,
-                        int ngram, int bits, int dtype, const uint64_t *scratch_key, const uint32_t *scratch_tf,
-                        int32_t *row_nnz, int64_t *indptr /*[dev] n_docs+1*/, int32_t *indices /*[dev] total*/,
-                        double *val64 /*[dev] total or NULL*/, float *val32 /*[dev] total*/,
-                        uint64_t *vocab_keys /*[dev] total*/, int32_t *df /*[dev] total*/,
-                        int32_t *vocab_size /*[dev] 1*/, int64_t *nnz_total /*[dev] 1*/, void *ws /*[dev]*/,
-                        size_t ws_bytes, void *stream);
+size_t sg_tfidf64_vocab_workspace_bytes(int64_t n_docs, int64_t total_symbols);
+int sg_tfidf64_vocab(const int64_t *offsets /*[dev]*/, int64_t n_docs, int64_t total_symbols, int ngram, int bits,
+                     const uint64_t *scratch_key, int32_t *row_nnz, int64_t *indptr /*[dev] n_docs+1*/,
+                     int32_t *indices /*[dev] total*/, uint64_t *vocab_keys /*[dev] total*/,
+                     int32_t *df /*[dev] total*/, int32_t *vocab_size /*[dev] 1*/, int64_t *nnz_total /*[dev] 1*/,
+                     void *ws /*[dev]*/, size_t ws_bytes, void *stream);
+int sg_tfidf64_values(const int64_t *offsets /*[dev]*/, int64_t n_docs, int dtype,
+                      const void *idf /*[dev] V, matrix dtype*/, const uint32_t *scratch_tf,
+                      const int64_t *indptr /*[dev] n_docs+1*/, const int32_t *indices /*[dev] total*/,
+                      double *val64 /*[dev] total or NULL*/, float *val32 /*[dev] total*/, void *stream);
 
 /* ------------------------------------------------------------------------- *
  * K2 — blocked CSR x CSR^T, thresholded, top-n per left row.
@@ -542,7 +549,9 @@ int sg_gather_bytes(const uint8_t *bytes /*[dev]*/, const int64_t *offsets /*[de
                     int64_t n_sel, const int32_t *positions /*[dev]*/, const int64_t *out_offsets /*[dev]*/,
                     uint8_t *out_bytes /*[dev]*/, void *stream);
 
-/* row-wise dot of two CSR matrices of equal shape (StringGrouper.dot, sg.py:433-440) */
+/* row-wise dot of two CSR matrices of equal shape (StringGrouper.dot, sg.py:433-440), summed in the reference's order:
+ * master.multiply(dup).sum(axis=1) = p0 + numpy's pairwise sum of p1..pk-1 over the common features, in the matrix
+ * dtype, no FMA */
 int sg_rowwise_dot(int64_t n_rows, const int64_t *a_indptr, const int32_t *a_indices, const void *a_val,
                    const int64_t *b_indptr, const int32_t *b_indices, const void *b_val, int dtype,
                    double *out /*[dev] n_rows*/, void *stream);

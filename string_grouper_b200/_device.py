@@ -1308,12 +1308,37 @@ def rowwise_dot(A, B):
     return out[:A.shape[0]].cpu().numpy().astype(A.dtype, copy=False)
 
 
-class DeviceVocabulary:
-    """df / rank tables of the fitted vectoriser (the device twin of TfidfVectorizer.vocabulary_ / idf_)."""
+def sklearn_idf(df, n_docs_fit, dtype):
+    """idf of every column, exactly as scikit-learn's TfidfTransformer.fit (smooth_idf=True) computes it from the
+    document frequencies `df` (column order) of `n_docs_fit` documents: the same four numpy statements on an array
+    of the matrix dtype.  The idf is computed on the host because numpy picks its `log` by CPU dispatch; no device
+    `log` gives the same bits."""
+    dtype = np.float32 if np.dtype(dtype) == np.float32 else np.float64
+    df = np.asarray(df).astype(dtype)
+    df += 1.0
+    idf = np.full_like(df, fill_value=int(n_docs_fit) + 1, dtype=dtype)
+    idf /= df
+    np.log(idf, out=idf)
+    idf += 1.0
+    return idf
 
-    def __init__(self, df_table, rank_table, ngram, n_docs, vocab_size):
+
+def _upload_idf(df_host, n_docs_fit, np_dtype, device):
+    """(host idf, device idf): sklearn_idf of the column-order df, copied to the device in the matrix dtype."""
+    idf = sklearn_idf(df_host, n_docs_fit, np_dtype)
+    TRANSFER_BYTES["h2d"] += int(idf.nbytes)
+    d_idf = torch().from_numpy(idf).to(device) if len(idf) else _empty(1, torch().float64, device)
+    return idf, d_idf
+
+
+class DeviceVocabulary:
+    """df / rank tables of the fitted vectoriser (the device twin of TfidfVectorizer.vocabulary_); `idf_` is the
+    twin of TfidfVectorizer.idf_ (numpy, matrix dtype)."""
+
+    def __init__(self, df_table, rank_table, ngram, n_docs, vocab_size, idf=None):
         self.d_df, self.d_rank = df_table, rank_table
         self.ngram, self.n_docs, self.size = int(ngram), int(n_docs), int(vocab_size)
+        self.idf_ = idf
 
     def feature_names(self):
         """Sorted n-grams, column order of the TF-IDF matrices (sklearn get_feature_names_out)."""
@@ -1339,9 +1364,10 @@ def upload_strings(data, offsets, device=None):
 class DeviceVocabulary64:
     """Sorted vocabulary of the general vectoriser (csrc/sg_tfidf64.cu): 64-bit keys over a dense alphabet."""
 
-    def __init__(self, keys, df, alphabet, bits, ngram, n_docs, vocab_size):
+    def __init__(self, keys, df, alphabet, bits, ngram, n_docs, vocab_size, idf=None):
         self.d_keys, self.d_df, self.alphabet = keys, df, alphabet
         self.bits, self.ngram, self.n_docs, self.size = int(bits), int(ngram), int(n_docs), int(vocab_size)
+        self.idf_ = idf
 
     def feature_names(self):
         from ._ingest import decode_vocab_keys64
@@ -1395,21 +1421,24 @@ def tfidf_sorted(data, offsets, n_master, ngram, flags, dtype, device=None, stat
     vocab_keys = _empty(total, t.int64, device)
     df = _empty(total, t.int32, device)
     tail = t.zeros(2, dtype=t.int64, device=device)         # [0] V (int32 view), [1] nnz
-    ws_bytes = int(L.sg_tfidf64_finalize_workspace_bytes(n_docs, total))
+    ws_bytes = int(L.sg_tfidf64_vocab_workspace_bytes(n_docs, total))
     ws = _empty(ws_bytes, t.uint8, device)
     dt = _lib.SG_DTYPE_F32 if np_dtype == np.float32 else _lib.SG_DTYPE_F64
-    _lib.check(L.sg_tfidf64_finalize(_ptr(d_off), n_docs, n_docs, total, int(ngram), bits, dt, _ptr(s_key), _ptr(s_tf),
-                                     _ptr(row_nnz), _ptr(indptr), _ptr(indices), _ptr(val64), _ptr(val32),
-                                     _ptr(vocab_keys), _ptr(df), ctypes.c_void_p(tail.data_ptr()),
-                                     ctypes.c_void_p(tail.data_ptr() + 8), _ptr(ws), ws_bytes, _stream()))
-    LAUNCH_COUNTS["tfidf"] += 7
+    _lib.check(L.sg_tfidf64_vocab(_ptr(d_off), n_docs, total, int(ngram), bits, _ptr(s_key), _ptr(row_nnz),
+                                  _ptr(indptr), _ptr(indices), _ptr(vocab_keys), _ptr(df),
+                                  ctypes.c_void_p(tail.data_ptr()), ctypes.c_void_p(tail.data_ptr() + 8), _ptr(ws),
+                                  ws_bytes, _stream()))
     n_master = int(n_master)
-    head = t.cat([tail, indptr[n_master:n_master + 1]]).cpu().numpy()
+    head = t.cat([tail, indptr[n_master:n_master + 1]]).cpu().numpy()     # V, nnz, split point
     V = int(head[0:1].view(np.int32)[0])
     nnz = int(head[1])
     split = int(head[2])
+    idf, d_idf = _upload_idf(to_host(df[:V])[0], n_docs, np_dtype, device)
+    _lib.check(L.sg_tfidf64_values(_ptr(d_off), n_docs, dt, _ptr(d_idf), _ptr(s_tf), _ptr(indptr), _ptr(indices),
+                                   _ptr(val64), _ptr(val32), _stream()))
+    LAUNCH_COUNTS["tfidf"] += 7
     val = val64 if np_dtype == np.float64 else val32
-    vocab = DeviceVocabulary64(vocab_keys, df, alphabet, bits, ngram, n_docs, V)
+    vocab = DeviceVocabulary64(vocab_keys, df, alphabet, bits, ngram, n_docs, V, idf)
     if stats is not None:
         stats.update(n_docs=n_docs, total_bytes=total, nnz=nnz, vocab=V, h2d_bytes=int(total * sym_width + 8 * len(offsets)),
                      vectoriser="sorted vocabulary, %d-bit keys" % (int(ngram) * bits))
@@ -1473,22 +1502,27 @@ def tfidf_resident(d_bytes, d_off, n_docs, total, n_master, ngram, flags, dtype,
     val32 = _empty(total, t.float32, device)
     val64 = _empty(total, t.float64, device) if np_dtype == np.float64 else None
     tail = t.zeros(2, dtype=t.int64, device=device)         # [0] V (int32 view), [1] nnz
-    ws_bytes = int(L.sg_tfidf_finalize_workspace_bytes(n_docs, int(ngram)))
+    ws_bytes = int(L.sg_tfidf_vocab_workspace_bytes(n_docs, int(ngram)))
     ws = _empty(ws_bytes, t.uint8, device)
     dt = _lib.SG_DTYPE_F32 if np_dtype == np.float32 else _lib.SG_DTYPE_F64
-    _lib.check(L.sg_tfidf_finalize(_ptr(d_off), n_docs, int(n_docs if n_docs_fit is None else n_docs_fit), int(ngram),
-                                   dt, _ptr(df), _ptr(rank), _ptr(s_key), _ptr(s_tf),
-                                   _ptr(row_nnz), _ptr(indptr), _ptr(indices), _ptr(val64), _ptr(val32),
-                                   ctypes.c_void_p(tail.data_ptr()), ctypes.c_void_p(tail.data_ptr() + 8), _ptr(ws),
-                                   ws_bytes, _stream()))
-    LAUNCH_COUNTS["tfidf"] += 4
+    _lib.check(L.sg_tfidf_vocab(n_docs, int(ngram), _ptr(df), _ptr(rank), _ptr(row_nnz), _ptr(indptr),
+                                ctypes.c_void_p(tail.data_ptr()), ctypes.c_void_p(tail.data_ptr() + 8), _ptr(ws),
+                                ws_bytes, _stream()))
     n_master = int(n_master)
-    head = t.cat([tail, indptr[n_master:n_master + 1]]).cpu().numpy()     # one read-back: V, nnz, split point
+    head = t.cat([tail, indptr[n_master:n_master + 1]]).cpu().numpy()     # V, nnz, split point
     V = int(head[0:1].view(np.int32)[0])
     nnz = int(head[1])
     split = int(head[2])
+    # idf on the host from df in column order (sklearn_idf), then the values
+    n_fit = n_docs if n_docs_fit is None else int(n_docs_fit)
+    col_df = _empty(max(V, 1), t.int32, device)
+    _lib.check(L.sg_tfidf_vocab_df(_ptr(df), _ptr(rank), int(ngram), _ptr(col_df), _stream()))
+    idf, d_idf = _upload_idf(to_host(col_df[:V])[0], n_fit, np_dtype, device)
+    _lib.check(L.sg_tfidf_values(_ptr(d_off), n_docs, dt, _ptr(d_idf), _ptr(rank), _ptr(s_key), _ptr(s_tf),
+                                 _ptr(row_nnz), _ptr(indptr), _ptr(indices), _ptr(val64), _ptr(val32), _stream()))
+    LAUNCH_COUNTS["tfidf"] += 5
     val = val64 if np_dtype == np.float64 else val32
-    vocab = DeviceVocabulary(df, rank, ngram, n_docs if n_docs_fit is None else n_docs_fit, V)
+    vocab = DeviceVocabulary(df, rank, ngram, n_fit, V, idf)
     if stats is not None:
         stats.update(n_docs=n_docs, total_bytes=total, nnz=nnz, vocab=V)
     master = DeviceCSR((n_master, V), indptr[:n_master + 1], indices, val, val32, split, np_dtype, 1.0, base=0)
@@ -1496,8 +1530,6 @@ def tfidf_resident(d_bytes, d_off, n_docs, total, n_master, ngram, flags, dtype,
     if n_master == n_docs:
         if df_allreduce is None and n_docs_fit is None:
             # fitted on exactly these rows: the vectoriser's df, in column order, is sg_feature_df(master)
-            col_df = _empty(max(V, 1), t.int32, device)
-            _lib.check(L.sg_tfidf_vocab_df(_ptr(df), _ptr(rank), int(ngram), _ptr(col_df), _stream()))
             master._df = col_df
         return master, None, vocab
     dup = DeviceCSR((n_docs - n_master, V), indptr[n_master:], indices, val, val32, nnz - split, np_dtype, 1.0,

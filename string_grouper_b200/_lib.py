@@ -41,14 +41,15 @@ SIGNATURES = {
     "sg_device_info": (_i32, [_p, _p, _p]),
     "sg_tfidf_table_slots": (_i64, [_i32]),
     "sg_tfidf_count": (_i32, [_p, _p, _i64, _i32, _u32, _p, _p, _p, _p, _p, _p, _p]),
-    "sg_tfidf_finalize_workspace_bytes": (_sz, [_i64, _i32]),
-    "sg_tfidf_finalize": (_i32, [_p, _i64, _i64, _i32, _i32, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _sz, _p]),
+    "sg_tfidf_vocab_workspace_bytes": (_sz, [_i64, _i32]),
+    "sg_tfidf_vocab": (_i32, [_i64, _i32, _p, _p, _p, _p, _p, _p, _p, _sz, _p]),
+    "sg_tfidf_values": (_i32, [_p, _i64, _i32, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "sg_tfidf_vocab_keys": (_i32, [_p, _p, _i32, _p, _p]),
     "sg_tfidf_vocab_df": (_i32, [_p, _p, _i32, _p, _p]),
     "sg_tfidf64_count": (_i32, [_p, _i32, _p, _i64, _i32, _i32, _p, _p, _p, _p, _p, _p, _p]),
-    "sg_tfidf64_finalize_workspace_bytes": (_sz, [_i64, _i64]),
-    "sg_tfidf64_finalize": (_i32, [_p, _i64, _i64, _i64, _i32, _i32, _i32, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p,
-                                   _p, _p, _sz, _p]),
+    "sg_tfidf64_vocab_workspace_bytes": (_sz, [_i64, _i64]),
+    "sg_tfidf64_vocab": (_i32, [_p, _i64, _i64, _i32, _i32, _p, _p, _p, _p, _p, _p, _p, _p, _p, _sz, _p]),
+    "sg_tfidf64_values": (_i32, [_p, _i64, _i32, _p, _p, _p, _p, _p, _p, _p]),
     "sg_num_tiles": (_i64, [_i64, _i32]),
     "sg_num_tiles_padded": (_i64, [_i64, _i32]),
     "sg_postings_workspace_bytes": (_sz, [_i64, _i64, _i64]),

@@ -889,6 +889,63 @@ rescore_refined_kernel(int64_t n, const int32_t *__restrict__ cr, const int32_t 
     }
 }
 
+// The products of a row pair (common features in ascending order, each multiplied in T), one at a time.
+template <typename T>
+struct CommonProducts {
+    const int32_t *ai, *bi;
+    const T *av, *bv;
+    int64_t pa, ea, pb, eb;
+    __device__ __forceinline__ T next() {      // the caller knows how many there are
+        for (;;) {
+            const int32_t fa = ai[pa], fb = bi[pb];
+            if (fa == fb) return ExactOps<T>::mul(av[pa++], bv[pb++]);
+            if (fa < fb) ++pa; else ++pb;
+        }
+    }
+};
+
+template <typename T>
+__device__ int64_t count_common(const int32_t *__restrict__ ai, int64_t pa, int64_t ea,
+                                const int32_t *__restrict__ bi, int64_t pb, int64_t eb) {
+    int64_t k = 0;
+    while (pa < ea && pb < eb) {
+        const int32_t fa = ai[pa], fb = bi[pb];
+        k += fa == fb;
+        pa += fa <= fb;
+        pb += fb <= fa;
+    }
+    return k;
+}
+
+constexpr int PW_BLOCKSIZE = 128;     // numpy's pairwise-sum block (numpy/_core/src/umath/loops_utils.h.src)
+
+// numpy's pairwise sum of the next n (<= PW_BLOCKSIZE) products: a plain loop below 8 terms, else 8 accumulators over
+// the multiple of 8, combined as ((r0+r1)+(r2+r3))+((r4+r5)+(r6+r7)), then the rest one by one
+template <typename T>
+__device__ __forceinline__ T pairwise_block(CommonProducts<T> &p, int64_t n) {
+    T res = (T)0;
+    if (n < 8) {
+        for (int64_t i = 0; i < n; ++i) res = ExactOps<T>::add(res, p.next());
+        return res;
+    }
+    T r[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) r[j] = p.next();
+    int64_t i = 8;
+    for (; i < n - (n % 8); i += 8) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) r[j] = ExactOps<T>::add(r[j], p.next());
+    }
+    res = ExactOps<T>::add(ExactOps<T>::add(ExactOps<T>::add(r[0], r[1]), ExactOps<T>::add(r[2], r[3])),
+                           ExactOps<T>::add(ExactOps<T>::add(r[4], r[5]), ExactOps<T>::add(r[6], r[7])));
+    for (; i < n; ++i) res = ExactOps<T>::add(res, p.next());
+    return res;
+}
+
+// StringGrouper.dot = master.multiply(dup).sum(axis=1): scipy reduces a row with np.add.reduceat, i.e. p0 + numpy's
+// pairwise sum of p1..pk-1.  Above PW_BLOCKSIZE terms numpy splits n into n2 = n/2 rounded down to a multiple of 8 and
+// n - n2 and adds the two halves; the recursion runs here on an explicit stack of pending right halves (the leaves are
+// visited left to right, i.e. in the order the merge walk produces the products).
 template <typename T>
 __global__ void rowwise_dot_kernel(int64_t n, const int64_t *__restrict__ a_indptr,
                                    const int32_t *__restrict__ a_idx, const T *__restrict__ a_val,
@@ -896,8 +953,41 @@ __global__ void rowwise_dot_kernel(int64_t n, const int64_t *__restrict__ a_indp
                                    const T *__restrict__ b_val, double *__restrict__ out) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    out[i] = (double)merge_dot<T>(a_idx, a_val, a_indptr[i], a_indptr[i + 1], b_idx, b_val, b_indptr[i],
-                                  b_indptr[i + 1]);
+    const int64_t pa = a_indptr[i], ea = a_indptr[i + 1], pb = b_indptr[i], eb = b_indptr[i + 1];
+    const int64_t k = count_common<T>(a_idx, pa, ea, b_idx, pb, eb);
+    if (k == 0) {
+        out[i] = 0.0;
+        return;
+    }
+    CommonProducts<T> p{a_idx, b_idx, a_val, b_val, pa, ea, pb, eb};
+    const T p0 = p.next();
+    if (k == 1) {
+        out[i] = (double)p0;
+        return;
+    }
+    int64_t right[32];       // a row has fewer than 2^31 entries: at most 24 halvings down to a block
+    T left[32];
+    bool have_left[32];
+    int sp = 0;
+    int64_t m = k - 1;
+    T res;
+    for (;;) {
+        while (m > PW_BLOCKSIZE) {
+            int64_t m2 = m / 2;
+            m2 -= m2 % 8;
+            right[sp] = m - m2;
+            have_left[sp] = false;
+            ++sp;
+            m = m2;
+        }
+        res = pairwise_block<T>(p, m);
+        while (sp > 0 && have_left[sp - 1]) res = ExactOps<T>::add(left[--sp], res);
+        if (sp == 0) break;
+        left[sp - 1] = res;
+        have_left[sp - 1] = true;
+        m = right[sp - 1];
+    }
+    out[i] = (double)ExactOps<T>::add(p0, res);
 }
 
 // ---------------------------------------------------------------------------

@@ -14,8 +14,9 @@
 //   among the keys present is sklearn's sorted-vocabulary column id)  ->  sort the
 //   document's keys with a warp bitonic network  ->  run-length encode to
 //   (key, tf)  ->  df[key] += 1 per distinct key.
-// Then: rank = exclusive scan of (df > 0); idf, tf*idf, row L2 norm in double in
-// column order; indices / values written coalesced at indptr[doc].
+// Then (sg_tfidf_vocab): rank = exclusive scan of (df > 0), indptr, V, nnz; the host reads df in column order back and
+// computes idf exactly as scikit-learn does (numpy's log); (sg_tfidf_values) tf*idf, row L2 norm in double in column
+// order; indices / values written coalesced at indptr[doc].
 #include <cub/cub.cuh>
 
 #include "sg_common.cuh"
@@ -149,36 +150,28 @@ __global__ void tfidf_tail_kernel(int64_t slots, const int32_t *__restrict__ df,
 }
 
 template <typename T>
-struct IdfMath;
+struct NormMath;
 template <>
-struct IdfMath<double> {
-    static __device__ __forceinline__ double idf(int64_t n1, int32_t dfk) {
-        return log(__ddiv_rn((double)n1, (double)(dfk + 1))) + 1.0;
-    }
+struct NormMath<double> {
     static __device__ __forceinline__ double sq(double x) { return __dmul_rn(x, x); }
     static __device__ __forceinline__ double scale(double x, double norm) { return __ddiv_rn(x, norm); }
 };
 template <>
-struct IdfMath<float> {
-    static __device__ __forceinline__ float idf(int64_t n1, int32_t dfk) {
-        return __fadd_rn(logf(__fdiv_rn((float)n1, (float)(dfk + 1))), 1.0f);
-    }
+struct NormMath<float> {
     static __device__ __forceinline__ double sq(float x) { return (double)__fmul_rn(x, x); }
     static __device__ __forceinline__ float scale(float x, double norm) { return (float)__ddiv_rn((double)x, norm); }
 };
 
-// T = matrix dtype (tfidf_matrix_dtype, string_grouper.py:18).  Arithmetic follows sklearn:
-// idf = log(n/df)+1 in T; x = tf*idf in T; sum of squares in double in column order; x / sqrt(sum).
+// T = matrix dtype (tfidf_matrix_dtype, string_grouper.py:18).  Arithmetic follows sklearn: x = tf*idf in T (idf[V]
+// computed on the host by numpy, exactly TfidfTransformer.fit); sum of squares in double in column order; x / sqrt(sum).
 template <typename T>
 __global__ void __launch_bounds__(K1_WARPS * 32)
-tfidf_finalize_kernel(const int64_t *__restrict__ offsets, int64_t n_docs, int64_t n_docs_fit,
-                      const int32_t *__restrict__ df,
-                      const int32_t *__restrict__ rank, const uint32_t *__restrict__ scratch_key,
-                      const uint32_t *__restrict__ scratch_tf, const int32_t *__restrict__ row_nnz,
-                      const int64_t *__restrict__ indptr, int32_t *__restrict__ indices,
-                      double *__restrict__ val64, float *__restrict__ val32) {
+tfidf_values_kernel(const int64_t *__restrict__ offsets, int64_t n_docs, const T *__restrict__ idf,
+                    const int32_t *__restrict__ rank, const uint32_t *__restrict__ scratch_key,
+                    const uint32_t *__restrict__ scratch_tf, const int32_t *__restrict__ row_nnz,
+                    const int64_t *__restrict__ indptr, int32_t *__restrict__ indices,
+                    double *__restrict__ val64, float *__restrict__ val32) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int64_t n1 = n_docs_fit + 1;   // smooth_idf: one extra document (sklearn TfidfTransformer.fit)
     for (int64_t doc = (int64_t)blockIdx.x * K1_WARPS + warp; doc < n_docs; doc += (int64_t)gridDim.x * K1_WARPS) {
         const int nnz = row_nnz[doc];
         if (nnz == 0) continue;
@@ -188,19 +181,18 @@ tfidf_finalize_kernel(const int64_t *__restrict__ offsets, int64_t n_docs, int64
             const int i = base + lane;
             double sq = 0.0;
             if (i < nnz) {
-                const uint32_t key = scratch_key[s + i];
-                const T x = (T)scratch_tf[s + i] * IdfMath<T>::idf(n1, df[key]);
-                sq = IdfMath<T>::sq(x);
+                const T x = (T)scratch_tf[s + i] * idf[rank[scratch_key[s + i]]];
+                sq = NormMath<T>::sq(x);
             }
             const int m = nnz - base < 32 ? nnz - base : 32;
             for (int l = 0; l < m; ++l) sum = __dadd_rn(sum, __shfl_sync(FULL, sq, l));
         }
         const double norm = __dsqrt_rn(sum);
         for (int i = lane; i < nnz; i += 32) {
-            const uint32_t key = scratch_key[s + i];
-            T x = (T)scratch_tf[s + i] * IdfMath<T>::idf(n1, df[key]);
-            if (sum != 0.0) x = IdfMath<T>::scale(x, norm);
-            indices[o + i] = rank[key];
+            const int32_t c = rank[scratch_key[s + i]];
+            T x = (T)scratch_tf[s + i] * idf[c];
+            if (sum != 0.0) x = NormMath<T>::scale(x, norm);
+            indices[o + i] = c;
             if (val64) val64[o + i] = (double)x;
             val32[o + i] = (float)x;
         }
@@ -248,7 +240,7 @@ int sg_tfidf_count(const uint8_t *bytes, const int64_t *offsets, int64_t n_docs,
     return SG_OK;
 }
 
-size_t sg_tfidf_finalize_workspace_bytes(int64_t n_docs, int ngram) {
+size_t sg_tfidf_vocab_workspace_bytes(int64_t n_docs, int ngram) {
     const int64_t slots = sg_tfidf_table_slots(ngram);
     if (slots < 0) return 0;
     size_t b1 = 0, b2 = 0;
@@ -258,17 +250,13 @@ size_t sg_tfidf_finalize_workspace_bytes(int64_t n_docs, int ngram) {
     return align_up((size_t)slots * 4, 256) + align_up(b1 > b2 ? b1 : b2, 256) + 1024;
 }
 
-int sg_tfidf_finalize(const int64_t *offsets, int64_t n_docs, int64_t n_docs_fit, int ngram, int dtype,
-                      const int32_t *df_table,
-                      int32_t *rank_table, const uint32_t *scratch_key, const uint32_t *scratch_tf,
-                      int32_t *row_nnz, int64_t *indptr, int32_t *indices, double *val64, float *val32,
-                      int32_t *vocab_size, int64_t *nnz_total, void *ws, size_t ws_bytes, void *stream_) {
+int sg_tfidf_vocab(int64_t n_docs, int ngram, const int32_t *df_table, int32_t *rank_table, int32_t *row_nnz,
+                   int64_t *indptr, int32_t *vocab_size, int64_t *nnz_total, void *ws, size_t ws_bytes,
+                   void *stream_) {
     cudaStream_t st = (cudaStream_t)stream_;
     const int64_t slots = sg_tfidf_table_slots(ngram);
     if (slots < 0) return fail(SG_ERR_UNSUPPORTED, "ngram_size %d unsupported (1..4)", ngram);
-    if (dtype != SG_DTYPE_F32 && dtype != SG_DTYPE_F64) return fail(SG_ERR_INVALID, "bad dtype");
-    if (dtype == SG_DTYPE_F64 && !val64) return fail(SG_ERR_INVALID, "val64 is required for float64");
-    if (n_docs < 0 || n_docs_fit < n_docs) return fail(SG_ERR_INVALID, "need 0 <= n_docs <= n_docs_fit");
+    if (n_docs < 0) return fail(SG_ERR_INVALID, "need n_docs >= 0");
     Arena ar(ws, ws_bytes);
     int32_t *flag = ar.take<int32_t>((size_t)slots);
     size_t b1 = 0, b2 = 0;
@@ -288,23 +276,31 @@ int sg_tfidf_finalize(const int64_t *offsets, int64_t n_docs, int64_t n_docs_fit
     SG_CUDA_TRY(cub::DeviceScan::ExclusiveSum(cub_tmp, cub_bytes, flag, rank_table, slots, st));
     tfidf_tail_kernel<<<1, 32, 0, st>>>(slots, df_table, rank_table, n_docs, indptr, vocab_size, nnz_total);
     SG_LAUNCH_CHECK();
-    if (n_docs > 0) {
-        int dev = 0, n_sm = 0;
-        SG_CUDA_TRY(cudaGetDevice(&dev));
-        SG_CUDA_TRY(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
-        int64_t grid = (n_docs + K1_WARPS - 1) / K1_WARPS;
-        const int64_t cap = (int64_t)n_sm * 8;
-        if (grid > cap) grid = cap;
-        if (dtype == SG_DTYPE_F64)
-            tfidf_finalize_kernel<double><<<(unsigned)grid, K1_WARPS * 32, 0, st>>>(
-                offsets, n_docs, n_docs_fit, df_table, rank_table, scratch_key, scratch_tf, row_nnz, indptr, indices,
-                val64, val32);
-        else
-            tfidf_finalize_kernel<float><<<(unsigned)grid, K1_WARPS * 32, 0, st>>>(
-                offsets, n_docs, n_docs_fit, df_table, rank_table, scratch_key, scratch_tf, row_nnz, indptr, indices,
-                nullptr, val32);
-        SG_LAUNCH_CHECK();
-    }
+    return SG_OK;
+}
+
+int sg_tfidf_values(const int64_t *offsets, int64_t n_docs, int dtype, const void *idf, const int32_t *rank_table,
+                    const uint32_t *scratch_key, const uint32_t *scratch_tf, const int32_t *row_nnz,
+                    const int64_t *indptr, int32_t *indices, double *val64, float *val32, void *stream_) {
+    cudaStream_t st = (cudaStream_t)stream_;
+    if (dtype != SG_DTYPE_F32 && dtype != SG_DTYPE_F64) return fail(SG_ERR_INVALID, "bad dtype");
+    if (dtype == SG_DTYPE_F64 && !val64) return fail(SG_ERR_INVALID, "val64 is required for float64");
+    if (n_docs <= 0) return SG_OK;
+    int dev = 0, n_sm = 0;
+    SG_CUDA_TRY(cudaGetDevice(&dev));
+    SG_CUDA_TRY(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
+    int64_t grid = (n_docs + K1_WARPS - 1) / K1_WARPS;
+    const int64_t cap = (int64_t)n_sm * 8;
+    if (grid > cap) grid = cap;
+    if (dtype == SG_DTYPE_F64)
+        tfidf_values_kernel<double><<<(unsigned)grid, K1_WARPS * 32, 0, st>>>(
+            offsets, n_docs, (const double *)idf, rank_table, scratch_key, scratch_tf, row_nnz, indptr, indices, val64,
+            val32);
+    else
+        tfidf_values_kernel<float><<<(unsigned)grid, K1_WARPS * 32, 0, st>>>(
+            offsets, n_docs, (const float *)idf, rank_table, scratch_key, scratch_tf, row_nnz, indptr, indices,
+            nullptr, val32);
+    SG_LAUNCH_CHECK();
     return SG_OK;
 }
 

@@ -154,17 +154,17 @@ __global__ void tfidf64_heads_kernel(int64_t n, const int64_t *__restrict__ nnz_
     if (i < n) head[i] = (i < *nnz_ptr && (i == 0 || keys_sorted[i] != keys_sorted[i - 1])) ? 1 : 0;
 }
 
-// col_scan = inclusive scan of head; column of sorted position i = col_scan[i] - 1
+// col_scan = inclusive scan of head; column of sorted position i = col_scan[i] - 1, written to the entry's CSR slot
 __global__ void tfidf64_columns_kernel(const int64_t *__restrict__ nnz_ptr, const uint64_t *__restrict__ keys_sorted,
                                        const uint32_t *__restrict__ pos_sorted, const int32_t *__restrict__ head,
-                                       const int32_t *__restrict__ col_scan, int32_t *__restrict__ col_of_entry,
+                                       const int32_t *__restrict__ col_scan, int32_t *__restrict__ indices,
                                        uint64_t *__restrict__ vocab_keys, int32_t *__restrict__ head_pos,
                                        int32_t *__restrict__ vocab_size) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const int64_t nnz = *nnz_ptr;
     if (i >= nnz) return;
     const int c = col_scan[i] - 1;
-    col_of_entry[pos_sorted[i]] = c;
+    indices[pos_sorted[i]] = c;
     if (head[i]) {
         vocab_keys[c] = keys_sorted[i];
         head_pos[c] = (int32_t)i;
@@ -182,34 +182,26 @@ __global__ void tfidf64_df_kernel(const int32_t *__restrict__ vocab_size, const 
 }
 
 template <typename T>
-struct IdfMath64;
+struct NormMath64;
 template <>
-struct IdfMath64<double> {
-    static __device__ __forceinline__ double idf(int64_t n1, int32_t dfk) {
-        return log(__ddiv_rn((double)n1, (double)(dfk + 1))) + 1.0;
-    }
+struct NormMath64<double> {
     static __device__ __forceinline__ double sq(double x) { return __dmul_rn(x, x); }
     static __device__ __forceinline__ double scale(double x, double norm) { return __ddiv_rn(x, norm); }
 };
 template <>
-struct IdfMath64<float> {
-    static __device__ __forceinline__ float idf(int64_t n1, int32_t dfk) {
-        return __fadd_rn(logf(__fdiv_rn((float)n1, (float)(dfk + 1))), 1.0f);
-    }
+struct NormMath64<float> {
     static __device__ __forceinline__ double sq(float x) { return (double)__fmul_rn(x, x); }
     static __device__ __forceinline__ float scale(float x, double norm) { return (float)__ddiv_rn((double)x, norm); }
 };
 
-// same arithmetic as tfidf_finalize_kernel (sklearn: idf in T, x = tf*idf in T, squares summed in double in column
-// order, x / sqrt(sum)); the column and df of an entry come from the sorted vocabulary
+// same arithmetic as tfidf_values_kernel (sklearn: x = tf*idf in T with the host's idf[V], squares summed in double in
+// column order, x / sqrt(sum)); the column of an entry is already in indices (sg_tfidf64_vocab)
 template <typename T>
 __global__ void __launch_bounds__(K64_WARPS * 32)
-tfidf64_finalize_kernel(const int64_t *__restrict__ offsets, int64_t n_docs, int64_t n_docs_fit,
-                        const int32_t *__restrict__ df, const int32_t *__restrict__ col_of_entry,
-                        const uint32_t *__restrict__ scratch_tf, const int64_t *__restrict__ indptr,
-                        int32_t *__restrict__ indices, double *__restrict__ val64, float *__restrict__ val32) {
+tfidf64_values_kernel(const int64_t *__restrict__ offsets, int64_t n_docs, const T *__restrict__ idf,
+                      const uint32_t *__restrict__ scratch_tf, const int64_t *__restrict__ indptr,
+                      const int32_t *__restrict__ indices, double *__restrict__ val64, float *__restrict__ val32) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int64_t n1 = n_docs_fit + 1;
     for (int64_t doc = (int64_t)blockIdx.x * K64_WARPS + warp; doc < n_docs; doc += (int64_t)gridDim.x * K64_WARPS) {
         const int64_t s = offsets[doc], o = indptr[doc];
         const int nnz = (int)(indptr[doc + 1] - o);
@@ -219,18 +211,16 @@ tfidf64_finalize_kernel(const int64_t *__restrict__ offsets, int64_t n_docs, int
             const int i = base + lane;
             double sq = 0.0;
             if (i < nnz) {
-                const T x = (T)scratch_tf[s + i] * IdfMath64<T>::idf(n1, df[col_of_entry[o + i]]);
-                sq = IdfMath64<T>::sq(x);
+                const T x = (T)scratch_tf[s + i] * idf[indices[o + i]];
+                sq = NormMath64<T>::sq(x);
             }
             const int m = nnz - base < 32 ? nnz - base : 32;
             for (int l = 0; l < m; ++l) sum = __dadd_rn(sum, __shfl_sync(FULL, sq, l));
         }
         const double norm = __dsqrt_rn(sum);
         for (int i = lane; i < nnz; i += 32) {
-            const int c = col_of_entry[o + i];
-            T x = (T)scratch_tf[s + i] * IdfMath64<T>::idf(n1, df[c]);
-            if (sum != 0.0) x = IdfMath64<T>::scale(x, norm);
-            indices[o + i] = c;
+            T x = (T)scratch_tf[s + i] * idf[indices[o + i]];
+            if (sum != 0.0) x = NormMath64<T>::scale(x, norm);
             if (val64) val64[o + i] = (double)x;
             val32[o + i] = (float)x;
         }
@@ -279,7 +269,7 @@ int sg_tfidf64_count(const void *symbols, int sym_width, const int64_t *offsets,
     return SG_OK;
 }
 
-size_t sg_tfidf64_finalize_workspace_bytes(int64_t n_docs, int64_t total_symbols) {
+size_t sg_tfidf64_vocab_workspace_bytes(int64_t n_docs, int64_t total_symbols) {
     const int64_t n = total_symbols < 1 ? 1 : total_symbols;
     size_t b1 = 0, b2 = 0, b3 = 0;
     cub::DeviceScan::ExclusiveScan(nullptr, b1, (int32_t *)nullptr, (int64_t *)nullptr, cub::Sum(), (int64_t)0,
@@ -289,23 +279,20 @@ size_t sg_tfidf64_finalize_workspace_bytes(int64_t n_docs, int64_t total_symbols
     cub::DeviceScan::InclusiveSum(nullptr, b3, (int32_t *)nullptr, (int32_t *)nullptr, n);
     size_t cubb = b1 > b2 ? b1 : b2;
     cubb = cubb > b3 ? cubb : b3;
-    return 2 * align_up((size_t)n * 8, 256) + 5 * align_up((size_t)(n + 2) * 4, 256) + align_up(cubb, 256) + 4096;
+    return 2 * align_up((size_t)n * 8, 256) + 4 * align_up((size_t)(n + 2) * 4, 256) + align_up(cubb, 256) + 4096;
 }
 
 /*
- * indptr, vocabulary (sorted distinct keys -> column ids, df), values.  `bits` bounds the sort.  Outputs: indptr,
- * indices, val64 (NULL for f32), val32, vocab_keys [total_symbols] (first V entries valid), df [total_symbols]
- * (first V valid), vocab_size, nnz_total.
+ * indptr, vocabulary (sorted distinct keys -> column ids, df).  `bits` bounds the sort.  Outputs: indptr, indices (the
+ * column of every entry), vocab_keys [total_symbols] (first V entries valid), df [total_symbols] (first V valid),
+ * vocab_size, nnz_total.
  */
-int sg_tfidf64_finalize(const int64_t *offsets, int64_t n_docs, int64_t n_docs_fit, int64_t total_symbols, int ngram,
-                        int bits, int dtype, const uint64_t *scratch_key, const uint32_t *scratch_tf, int32_t *row_nnz,
-                        int64_t *indptr, int32_t *indices, double *val64, float *val32, uint64_t *vocab_keys,
-                        int32_t *df, int32_t *vocab_size, int64_t *nnz_total, void *ws, size_t ws_bytes,
-                        void *stream_) {
+int sg_tfidf64_vocab(const int64_t *offsets, int64_t n_docs, int64_t total_symbols, int ngram, int bits,
+                     const uint64_t *scratch_key, int32_t *row_nnz, int64_t *indptr, int32_t *indices,
+                     uint64_t *vocab_keys, int32_t *df, int32_t *vocab_size, int64_t *nnz_total, void *ws,
+                     size_t ws_bytes, void *stream_) {
     cudaStream_t st = (cudaStream_t)stream_;
-    if (dtype != SG_DTYPE_F32 && dtype != SG_DTYPE_F64) return fail(SG_ERR_INVALID, "bad dtype");
-    if (dtype == SG_DTYPE_F64 && !val64) return fail(SG_ERR_INVALID, "val64 is required for float64");
-    if (n_docs < 0 || n_docs_fit < n_docs) return fail(SG_ERR_INVALID, "need 0 <= n_docs <= n_docs_fit");
+    if (n_docs < 0) return fail(SG_ERR_INVALID, "need n_docs >= 0");
     if (total_symbols >= (int64_t)0x7fffffff) return fail(SG_ERR_OVERFLOW, "corpus too large for int32 positions");
     const int64_t n = total_symbols < 1 ? 1 : total_symbols;
     Arena ar(ws, ws_bytes);
@@ -315,7 +302,6 @@ int sg_tfidf64_finalize(const int64_t *offsets, int64_t n_docs, int64_t n_docs_f
     uint32_t *pos_sorted = ar.take<uint32_t>((size_t)n + 2);
     int32_t *head = ar.take<int32_t>((size_t)n + 2);
     int32_t *col_scan = ar.take<int32_t>((size_t)n + 2);
-    int32_t *col_of_entry = ar.take<int32_t>((size_t)n + 2);
     size_t b1 = 0, b2 = 0, b3 = 0;
     cub::DeviceScan::ExclusiveScan(nullptr, b1, (int32_t *)nullptr, (int64_t *)nullptr, cub::Sum(), (int64_t)0,
                                    n_docs + 1);
@@ -350,25 +336,34 @@ int sg_tfidf64_finalize(const int64_t *offsets, int64_t n_docs, int64_t n_docs_f
         tfidf64_heads_kernel<<<g, 256, 0, st>>>(n, indptr + n_docs, keys_sorted, head);
         SG_LAUNCH_CHECK();
         SG_CUDA_TRY(cub::DeviceScan::InclusiveSum(tmp, cubb, head, col_scan, n, st));
-        tfidf64_columns_kernel<<<g, 256, 0, st>>>(indptr + n_docs, keys_sorted, pos_sorted, head, col_scan, col_of_entry,
+        tfidf64_columns_kernel<<<g, 256, 0, st>>>(indptr + n_docs, keys_sorted, pos_sorted, head, col_scan, indices,
                                                   vocab_keys, head_pos, vocab_size);
         SG_LAUNCH_CHECK();
         tfidf64_df_kernel<<<g, 256, 0, st>>>(vocab_size, head_pos, df, n);
         SG_LAUNCH_CHECK();
-        int dev = 0, n_sm = 0;
-        SG_CUDA_TRY(cudaGetDevice(&dev));
-        SG_CUDA_TRY(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
-        int64_t grid = (n_docs + K64_WARPS - 1) / K64_WARPS;
-        const int64_t cap = (int64_t)n_sm * 8;
-        if (grid > cap) grid = cap;
-        if (dtype == SG_DTYPE_F64)
-            tfidf64_finalize_kernel<double><<<(unsigned)grid, K64_WARPS * 32, 0, st>>>(
-                offsets, n_docs, n_docs_fit, df, col_of_entry, scratch_tf, indptr, indices, val64, val32);
-        else
-            tfidf64_finalize_kernel<float><<<(unsigned)grid, K64_WARPS * 32, 0, st>>>(
-                offsets, n_docs, n_docs_fit, df, col_of_entry, scratch_tf, indptr, indices, nullptr, val32);
-        SG_LAUNCH_CHECK();
     }
+    return SG_OK;
+}
+
+int sg_tfidf64_values(const int64_t *offsets, int64_t n_docs, int dtype, const void *idf, const uint32_t *scratch_tf,
+                      const int64_t *indptr, const int32_t *indices, double *val64, float *val32, void *stream_) {
+    cudaStream_t st = (cudaStream_t)stream_;
+    if (dtype != SG_DTYPE_F32 && dtype != SG_DTYPE_F64) return fail(SG_ERR_INVALID, "bad dtype");
+    if (dtype == SG_DTYPE_F64 && !val64) return fail(SG_ERR_INVALID, "val64 is required for float64");
+    if (n_docs <= 0) return SG_OK;
+    int dev = 0, n_sm = 0;
+    SG_CUDA_TRY(cudaGetDevice(&dev));
+    SG_CUDA_TRY(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
+    int64_t grid = (n_docs + K64_WARPS - 1) / K64_WARPS;
+    const int64_t cap = (int64_t)n_sm * 8;
+    if (grid > cap) grid = cap;
+    if (dtype == SG_DTYPE_F64)
+        tfidf64_values_kernel<double><<<(unsigned)grid, K64_WARPS * 32, 0, st>>>(
+            offsets, n_docs, (const double *)idf, scratch_tf, indptr, indices, val64, val32);
+    else
+        tfidf64_values_kernel<float><<<(unsigned)grid, K64_WARPS * 32, 0, st>>>(
+            offsets, n_docs, (const float *)idf, scratch_tf, indptr, indices, nullptr, val32);
+    SG_LAUNCH_CHECK();
     return SG_OK;
 }
 

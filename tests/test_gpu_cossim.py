@@ -236,15 +236,25 @@ def test_symmetrize_matches_lil_restatement():
     assert np.all(s[r == c] == 1.0) and (r == c).sum() == n
 
 
-def test_rowwise_dot():
+def _rowwise_dot_exact(dtype):
+    """bit-equal to the reference's dot() (scipy's p0 + numpy pairwise order, tests/exact_pipeline.py)"""
     from string_grouper_b200 import _device as D
     P = _oracle()
     a = make_names(1000, seed=7)
     b = make_names(1000, seed=7)[:500] + make_names(500, seed=8)
-    m, d, _ = P.tf_idf_matrices(a, b)
+    m, d, _ = P.tf_idf_matrices(a, b, dtype=dtype)
     ref = np.asarray(m.multiply(d).sum(axis=1)).squeeze(axis=1)
     got = D.rowwise_dot(D.DeviceCSR.from_scipy(m), D.DeviceCSR.from_scipy(d))
-    np.testing.assert_allclose(got, ref, atol=1e-12)
+    assert got.dtype == ref.dtype == dtype
+    assert np.array_equal(got, ref), "%d rows differ" % (got != ref).sum()
+
+
+def test_rowwise_dot():
+    _rowwise_dot_exact(np.float64)
+
+
+def test_rowwise_dot_float32():
+    _rowwise_dot_exact(np.float32)
 
 
 def test_nearest_master_matches_host_rule():

@@ -87,7 +87,7 @@ def test_full_size_all_pairs_equal_cpu_port(fitted):
     from string_grouper_b200 import _device as D
     names, sg = fitted
     A, _ = sg._get_tf_idf_matrices()
-    full = A.to_scipy()                 # equal to the sklearn matrix: tests/test_gpu_tfidf.py
+    full = A.to_scipy()                 # bit-equal to the sklearn matrix: tests/test_gpu_pipeline_exact.py (663k)
     C = P.build_matches(full, full, P.guess_blocks(N, N), 20, 0.8, _threads())
     S = P.symmetrize_fast(C)            # vectorised twin of the LIL restatement (tests/test_oracle.py)
     ml = P.matches_list(S)

@@ -1,5 +1,5 @@
-"""-m gpu: K1 (device n-gram TF-IDF) against sklearn driven by the reference analyzer (the oracle) and against
-the reference's own matrix stored in tests/golden/synthetic.npz."""
+"""-m gpu: K1 (device n-gram TF-IDF) against sklearn driven by the reference analyzer (the oracle), bit for bit, and
+against the reference's own matrix stored in tests/golden/synthetic.npz."""
 import os
 
 import numpy as np
@@ -21,16 +21,20 @@ def _device_matrices(master, dupes=None, **kw):
     return sg, m, d
 
 
-def _assert_same_csr(got, ref, rtol):
+def _assert_same_csr(got, ref):
+    """equal bit for bit: K1 computes idf with numpy on the host exactly as scikit-learn does"""
     got, ref = got.to_scipy(), ref.tocsr()
     assert got.shape == ref.shape
     assert np.array_equal(got.indptr, ref.indptr)
     assert np.array_equal(got.indices, ref.indices)
     assert got.dtype == ref.dtype
-    np.testing.assert_allclose(got.data, ref.data, rtol=rtol, atol=0)
+    assert np.array_equal(got.data, ref.data), "%d values differ" % (got.data != ref.data).sum()
 
 
 def test_matrix_equals_reference_golden():
+    """The golden matrix was written on another host: its idf carries that host's numpy `log` (picked by CPU
+    dispatch), which may differ from this host's in the last bit, so the values are compared with a tolerance here;
+    the exact comparisons are against live scikit-learn below."""
     texts = make_names(500, seed=14) + EDGE
     sg, m, _ = _device_matrices(texts)
     got = m.to_scipy()
@@ -55,9 +59,8 @@ def test_matrix_equals_sklearn_oracle(kw):
     okw = dict(kw)
     dtype = okw.pop("tfidf_matrix_dtype", np.float64)
     rm, rd, _ = P.tf_idf_matrices(master, dupes, dtype=dtype, **okw)
-    rtol = 1e-14 if dtype == np.float64 else 2e-6
-    _assert_same_csr(m, rm, rtol)
-    _assert_same_csr(d, rd, rtol)
+    _assert_same_csr(m, rm)
+    _assert_same_csr(d, rd)
 
 
 UNICODE = ["Caf\u00e9 M\u00fcller GmbH", "Cafe Muller GmbH", "CAF\u00c9 M\u00dcLLER GMBH", "\u6771\u4eac\u682a\u5f0f\u4f1a\u793e",
@@ -77,9 +80,8 @@ def test_code_point_ngrams_equal_sklearn_oracle(kw):
     okw = dict(kw)
     dtype = okw.pop("tfidf_matrix_dtype", np.float64)
     rm, rd, vec = P.tf_idf_matrices(master, dupes, dtype=dtype, normalize_to_ascii=False, **okw)
-    rtol = 1e-14 if dtype == np.float64 else 2e-6
-    _assert_same_csr(m, rm, rtol)
-    _assert_same_csr(d, rd, rtol)
+    _assert_same_csr(m, rm)
+    _assert_same_csr(d, rd)
     vocab = vec.vocabulary_
     assert sg._vocabulary.feature_names() == sorted(vocab, key=vocab.get)
 
@@ -107,7 +109,7 @@ def test_capital_ascii_from_nfkd_is_not_folded_again():
              "plain ascii"] + make_names(200, seed=36)
     sg, m, _ = _device_matrices(texts)
     rm, _, vec = P.tf_idf_matrices(texts)
-    _assert_same_csr(m, rm, 1e-14)
+    _assert_same_csr(m, rm)
     assert "eTM" in sg._vocabulary.feature_names()
 
 
