@@ -464,6 +464,42 @@ int sg_topn_select_rows(int64_t n_cand, const int32_t *cand_row, const int32_t *
                         void *stream);
 
 /*
+ * Self-match over groups of bit-identical rows (csrc/sg_dedup.cu, csrc/sg_select.cu; DESIGN.md §4 "Identical rows").
+ * sg_row_dedup: uid[n_rows] = group of every row; groups numbered by their first member, which is the representative
+ * rep[m]; members as a CSR over groups, mem_ptr[n_rows+1] (entries m..n_rows hold n_rows) and mem_rows[n_rows],
+ * ascending inside a group; out_sizes = {m, stored values of the representatives}.  A group's members are verified
+ * bit-identical (length, indices, value bits in `dtype`) to each other; the 64-bit row hash, masked by `hash_mask`
+ * (all ones in production), only orders the rows.
+ * sg_rows_gather: U = the rows rep[0..m) of a CSR matrix (out_indptr[m+1] from 0; out_val32 NULL: not copied).
+ */
+size_t sg_row_dedup_workspace_bytes(int64_t n_rows);
+int sg_row_dedup(int64_t n_rows, const int64_t *indptr, const int32_t *indices, const void *val, int dtype,
+                 uint64_t hash_mask, int32_t *uid, int32_t *mem_ptr, int32_t *mem_rows, int32_t *rep,
+                 int64_t *out_sizes /*[dev] 2*/, void *ws, size_t ws_bytes, void *stream);
+size_t sg_rows_gather_workspace_bytes(int64_t m);
+int sg_rows_gather(int64_t m, const int32_t *rep, const int64_t *indptr, const int32_t *indices, const void *val,
+                   const float *val32, int dtype, int64_t *out_indptr, int32_t *out_indices, void *out_val,
+                   float *out_val32, void *ws, size_t ws_bytes, void *stream);
+/*
+ * Selection of the product of U with itself, expanded to the original rows.  Input: sg_rescore's kept pairs in group
+ * space (u, v, score), mirrors included.  Every (u, v, s) stands for the pairs (u, c, s) of every member c of v; the
+ * survivors of u are ranked like sg_topn_select_rows ranks a row (score descending, the larger column wins a tie at
+ * the cut, ties written in ascending column order), and every row r gets a copy of the list of its group uid[r].
+ * sg_topn_groups_count: grp_cnt[m] = expanded survivors per group, totals = {sum of grp_cnt, output pairs} (the
+ * sizes the caller allocates).  Needs top_n <= sg_topn_rows_cap() / 2 when top_n > 32.
+ */
+int sg_topn_groups_count(int64_t n_cand, const int32_t *cand_row, const int32_t *cand_col, int64_t n_groups,
+                         const int32_t *mem_ptr, int top_n, int32_t *grp_cnt /*[dev] n_groups*/,
+                         int64_t *totals /*[dev] 2*/, void *stream);
+size_t sg_topn_select_groups_workspace_bytes(int64_t n_cand, int64_t n_expanded, int64_t n_groups, int64_t n_rows,
+                                             int top_n);
+int sg_topn_select_groups(int64_t n_cand, const int32_t *cand_row, const int32_t *cand_col, const double *score,
+                          int64_t n_groups, const int32_t *mem_ptr, const int32_t *mem_rows, const int32_t *grp_cnt,
+                          int64_t n_expanded, int64_t n_rows, const int32_t *uid, int top_n, int64_t *out_indptr,
+                          int32_t *out_row, int32_t *out_col, double *out_score, int64_t *out_nnz /*[dev] 1*/,
+                          int32_t *out_max_row /*[dev] 1*/, void *ws, size_t ws_bytes, void *stream);
+
+/*
  * K3 — per-row top-n merge of column-block results.  Replaces sparse_dot_topn.zip_sp_matmul_topn(top_n, C_mats)
  * (call site sg.py:746).  Input: the block results concatenated as COO (block column offsets already added, any
  * order); entries that are not strictly positive are dropped like the reference's heap does (its initial minimum

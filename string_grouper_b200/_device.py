@@ -14,7 +14,7 @@ _TORCH = None
 
 # hand-written kernels launched so far (CUB scans / sorts and memsets are not counted); bench.py "gpu_launches"
 LAUNCH_COUNTS = {"postings": 0, "candidates": 0, "rescore": 0, "select": 0, "symmetrize": 0, "tfidf": 0,
-                 "rowdot": 0, "order": 0, "tiles": 0, "groups": 0, "gather": 0, "prune": 0}
+                 "rowdot": 0, "order": 0, "tiles": 0, "groups": 0, "gather": 0, "prune": 0, "dedup": 0}
 # "tiles": the tile-centric K2 (csrc/sg_tiles.cu): build, pack_left, filter, candidates
 
 TRANSFER_BYTES = {"d2h": 0, "h2d": 0}      # bytes moved by the bulk copies (bench.py e2e accounting)
@@ -48,6 +48,11 @@ SELECT_MODE = os.environ.get("SG_B200_SELECT", "rows").lower()      # "rows" (pe
 # top-n floor (cossim_topn's `floor`): "auto" | "1" | "0"; auto considers it from FLOOR_MIN_ROWS left rows on
 TOPN_FLOOR = {"1": True, "0": False}.get(os.environ.get("SG_B200_TOPN_FLOOR", "auto").lower(), "auto")
 FLOOR_MIN_ROWS = 65536
+# dedup path of a self-match (cossim_topn's `dedup`): "auto" runs the product over the distinct rows from
+# DEDUP_MIN_ROWS rows on, when at least DEDUP_MIN_SHARE of the rows repeat another row bit for bit
+DEDUP_MIN_ROWS = 131072
+DEDUP_MIN_SHARE = 0.02
+DEDUP_HASH_MASK = (1 << 64) - 1       # row hash bits the grouping sorts by (tests narrow it to force collisions)
 
 
 def torch():
@@ -150,6 +155,7 @@ class DeviceCSR:
         self._df = None             # document frequency of every feature (sg_feature_df)
         self._heavy_norm = None     # per-row norm over the heavy features (sg_heavy_norms)
         self._heavy_groups = None   # the same per group of heavy ranks, fp16[16] (sg_rescore_refined)
+        self._dedup = None          # groups of bit-identical rows and the matrix of their representatives (row_groups)
         self.nonneg = True          # no negative stored value (K1 output; checked for uploaded matrices)
 
     @property
@@ -436,6 +442,57 @@ def feature_df(B):
     return B._df
 
 
+def row_groups(A):
+    """Groups of bit-identical rows of A (sg_row_dedup), cached on A: {"m", "uid", "mem_ptr", "mem_rows", "rep",
+    "nnz" (stored values of the representatives), "mask", "U" (unique_rows, once built)}."""
+    t = require_cuda()
+    L = _lib.load()
+    if A._dedup is None or A._dedup["mask"] != DEDUP_HASH_MASK:
+        n = A.shape[0]
+        uid = _empty(n, t.int32, A.device)
+        mem_ptr = _empty(n + 1, t.int32, A.device)
+        mem_rows = _empty(n, t.int32, A.device)
+        rep = _empty(n, t.int32, A.device)
+        sizes = t.zeros(2, dtype=t.int64, device=A.device)
+        ws_bytes = int(L.sg_row_dedup_workspace_bytes(n))
+        ws = _empty(ws_bytes, t.uint8, A.device)
+        _lib.check(L.sg_row_dedup(n, _ptr(A.d_indptr), _ptr(A.d_indices), _ptr(A.d_val),
+                                  _lib.SG_DTYPE_F32 if A.dtype == np.float32 else _lib.SG_DTYPE_F64,
+                                  DEDUP_HASH_MASK, _ptr(uid), _ptr(mem_ptr), _ptr(mem_rows), _ptr(rep), _ptr(sizes),
+                                  _ptr(ws), ws_bytes, _stream()))
+        LAUNCH_COUNTS["dedup"] += 6
+        m, nnz = (int(x) for x in sizes.cpu().numpy())
+        A._dedup = {"m": m, "uid": uid, "mem_ptr": mem_ptr, "mem_rows": mem_rows, "rep": rep, "nnz": nnz,
+                    "mask": DEDUP_HASH_MASK, "U": None}
+    return A._dedup
+
+
+def unique_rows(A):
+    """The matrix U of the representatives of row_groups(A) (row u = the first member of group u), cached on A; it
+    keeps A's norm bound and sign, so its product takes the same kernels and margins."""
+    t = require_cuda()
+    L = _lib.load()
+    g = row_groups(A)
+    if g["U"] is None:
+        m, nnz = g["m"], g["nnz"]
+        indptr = _empty(m + 1, t.int64, A.device)
+        indices = _empty(nnz, t.int32, A.device)
+        val = _empty(nnz, A.d_val.dtype, A.device)
+        val32 = val if A.d_val32 is A.d_val else _empty(nnz, t.float32, A.device)
+        ws_bytes = int(L.sg_rows_gather_workspace_bytes(m))
+        ws = _empty(ws_bytes, t.uint8, A.device)
+        _lib.check(L.sg_rows_gather(m, _ptr(g["rep"]), _ptr(A.d_indptr), _ptr(A.d_indices), _ptr(A.d_val),
+                                    None if val32 is val else _ptr(A.d_val32),
+                                    _lib.SG_DTYPE_F32 if A.dtype == np.float32 else _lib.SG_DTYPE_F64,
+                                    _ptr(indptr), _ptr(indices), _ptr(val), None if val32 is val else _ptr(val32),
+                                    _ptr(ws), ws_bytes, _stream()))
+        LAUNCH_COUNTS["dedup"] += 2
+        U = DeviceCSR((m, A.shape[1]), indptr, indices, val, val32, nnz, A.dtype, A.norm_bound)
+        U.nonneg = A.nonneg
+        g["U"] = U
+    return g["U"]
+
+
 def prune_left(A, B, hrank, row_begin, row_end, threshold, margin, margin_per_feature, frac):
     """Exact threshold pruning of rows [row_begin,row_end) of A against B (sg_prune_rows); only B's heavy
     features (hrank >= 0) are prunable.  Returns (indices, val32, row_len, row_threshold, pruned_norm,
@@ -479,7 +536,7 @@ def prune_left_floor(A, B, hrank, row_begin, row_end, threshold, margin, margin_
 
 
 def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, warps=None, stats=None,
-                prune=None, acc=None, kernel=None, floor=None):
+                prune=None, acc=None, kernel=None, floor=None, dedup=None):
     """C[i,:] = top_n{ j : A_i . B_j > threshold } for rows [row_begin,row_end) of A.
 
     Device counterpart of the whole block loop of StringGrouper._build_matches
@@ -491,6 +548,11 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
     24 bytes each exceed a quarter of device memory.  True needs top_n <= 32 and non-negative operands.  A threshold
     <= 0 (no threshold: every pair with a positive score counts) starts the floors from the exact scores of each
     row's neighbours in the processing order (topn_floor_init).
+
+    `dedup` (None = "auto"; True; False): a self-match over all rows on the usual path (not the floor), with the row
+    selection (SELECT_MODE "rows", top_n <= sg_topn_rows_cap() / 2), runs the product over the distinct rows U of A
+    and gives every row its group's list (DESIGN.md §4 "Identical rows"); the result is bit-identical.  "auto" takes it
+    from DEDUP_MIN_ROWS rows on when at least DEDUP_MIN_SHARE of them repeat another row; True wherever it applies.
     """
     t = require_cuda()
     L = _lib.load()
@@ -527,6 +589,22 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
             return out
     if stats is not None:
         stats["topn_floor"] = False
+
+    # Identical rows: the product over the distinct rows, expanded to every row by the selection (_select_groups)
+    if dedup not in (None, "auto", True, False):
+        raise ValueError("dedup must be None, 'auto', True or False, got %r" % (dedup,))
+    groups = None
+    if (dedup is not False and A is B and row_begin == 0 and row_end == n_left and SELECT_MODE == "rows"
+            and top_n <= int(L.sg_topn_rows_cap()) // 2 and (dedup is True or n_left >= DEDUP_MIN_ROWS)):
+        groups = row_groups(A)
+        if dedup is True or n_left - groups["m"] >= DEDUP_MIN_SHARE * n_left:
+            A = B = unique_rows(A)
+            n_left = n_right = row_end = n_rows = A.shape[0]
+        else:
+            groups = None
+        mark(stats, "dedup")
+    if stats is not None:
+        stats["dedup"] = groups is not None
 
     mark(stats, "k2_start")
     scale = A.norm_bound * B.norm_bound
@@ -820,6 +898,8 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
         if use_tiles:
             stats["stage_bytes"] = tiles["stage_bytes"]
 
+    if groups is not None:
+        return _select_groups(cand_row, cand_col, score, n_cand, groups, top_n, shape, stats)
     return _select_topn(cand_row, cand_col, score, n_cand, row_cnt, max_row_cnt, row_begin, n_rows, top_n, threshold,
                         shape, stats)
 
@@ -1181,6 +1261,41 @@ def _select_topn(cand_row, cand_col, score, n_cand, row_cnt, max_row_cnt, row_be
             stats["select"] = "sort"
     th = tail.cpu().numpy()
     mark(stats, "select")
+    nnz = int(th[0])
+    max_row = int(th[1:2].view(np.int32)[0])
+    return DeviceMatches(shape, out_row, out_col, out_score, nnz, max_row, indptr=out_indptr)
+
+
+def _select_groups(cand_row, cand_col, score, n_cand, groups, top_n, shape, stats):
+    """Top-n of every row from the re-scored survivors (u, v, score) of the product of U = unique_rows(A) with itself:
+    each (u, v) stands for u against every member of v, and every row gets its group's list (sg_topn_select_groups)."""
+    t = torch()
+    L = _lib.load()
+    dev = cand_row.device
+    m, n = groups["m"], shape[0]
+    grp_cnt = _empty(m, t.int32, dev)
+    totals = t.zeros(2, dtype=t.int64, device=dev)
+    _lib.check(L.sg_topn_groups_count(n_cand, _ptr(cand_row), _ptr(cand_col), m, _ptr(groups["mem_ptr"]), top_n,
+                                      _ptr(grp_cnt), _ptr(totals), _stream()))
+    n_expanded, n_out = (int(x) for x in totals.cpu().numpy())
+    out_indptr = _empty(n + 1, t.int64, dev)
+    out_row = _empty(n_out, t.int32, dev)
+    out_col = _empty(n_out, t.int32, dev)
+    out_score = _empty(n_out, t.float64, dev)
+    tail = t.zeros(2, dtype=t.int64, device=dev)            # [0] out_nnz, [1] max_row (int32 view)
+    ws_bytes = int(L.sg_topn_select_groups_workspace_bytes(n_cand, n_expanded, m, n, top_n))
+    ws = _empty(ws_bytes, t.uint8, dev)
+    _lib.check(L.sg_topn_select_groups(n_cand, _ptr(cand_row), _ptr(cand_col), _ptr(score), m, _ptr(groups["mem_ptr"]),
+                                       _ptr(groups["mem_rows"]), _ptr(grp_cnt), n_expanded, n, _ptr(groups["uid"]),
+                                       top_n, _ptr(out_indptr), _ptr(out_row), _ptr(out_col), _ptr(out_score),
+                                       ctypes.c_void_p(tail.data_ptr()), ctypes.c_void_p(tail.data_ptr() + 8),
+                                       _ptr(ws), ws_bytes, _stream()))
+    LAUNCH_COUNTS["select"] += 11 if top_n <= 32 else 13
+    th = tail.cpu().numpy()
+    mark(stats, "select")
+    if stats is not None:
+        stats["select"] = "rows"
+        stats["n_unique_rows"], stats["n_expanded"] = m, n_expanded
     nnz = int(th[0])
     max_row = int(th[1:2].view(np.int32)[0])
     return DeviceMatches(shape, out_row, out_col, out_score, nnz, max_row, indptr=out_indptr)

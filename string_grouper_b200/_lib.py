@@ -91,6 +91,14 @@ SIGNATURES = {
     "sg_row_count_max": (_i32, [_i64, _p, _p, _p]),
     "sg_topn_select_rows_workspace_bytes": (_sz, [_i64, _i64]),
     "sg_topn_select_rows": (_i32, [_i64, _p, _p, _p, _i64, _i64, _i32, _p, _p, _p, _p, _p, _p, _p, _p, _sz, _p]),
+    "sg_row_dedup_workspace_bytes": (_sz, [_i64]),
+    "sg_row_dedup": (_i32, [_i64, _p, _p, _p, _i32, ctypes.c_uint64, _p, _p, _p, _p, _p, _p, _sz, _p]),
+    "sg_rows_gather_workspace_bytes": (_sz, [_i64]),
+    "sg_rows_gather": (_i32, [_i64, _p, _p, _p, _p, _p, _i32, _p, _p, _p, _p, _p, _sz, _p]),
+    "sg_topn_groups_count": (_i32, [_i64, _p, _p, _i64, _p, _i32, _p, _p, _p]),
+    "sg_topn_select_groups_workspace_bytes": (_sz, [_i64, _i64, _i64, _i64, _i32]),
+    "sg_topn_select_groups": (_i32, [_i64, _p, _p, _p, _i64, _p, _p, _p, _i64, _i64, _p, _i32, _p, _p, _p, _p, _p, _p,
+                                     _p, _sz, _p]),
     "sg_topn_select_workspace_bytes": (_sz, [_i64, _i64]),
     "sg_topn_select": (_i32, [_i64, _p, _p, _p, _i64, _i64, _i32, _f64, _p, _p, _p, _p, _p, _p, _p, _sz, _p]),
     "sg_topn_merge_workspace_bytes": (_sz, [_i64, _i64]),

@@ -287,6 +287,149 @@ __global__ void sel_max_count_kernel(int64_t n_rows, const int32_t *__restrict__
     if ((threadIdx.x & 31) == 0 && m > 0) atomicMax(out, m);
 }
 
+// Ranks rows [0, n_rows) of the row buckets (row_start, b_col, b_score) into out_indptr's slots; big_rows has n_rows
+// entries, *n_big is zeroed by the caller.
+static int sel_rank_rows(int64_t n_rows, int64_t row_begin, const int64_t *row_start, const int32_t *b_col,
+                         const double *b_score, int top_n, const int64_t *out_indptr, int32_t *out_row,
+                         int32_t *out_col, double *out_score, int32_t *big_rows, int32_t *n_big, cudaStream_t st) {
+    if (top_n <= 32) {
+        // the common case (max_n_matches defaults to 20): every row, whatever its length, by one warp
+        sel_rows_small_kernel<true><<<(unsigned)((n_rows + 7) / 8), 256, 0, st>>>(
+            n_rows, row_begin, row_start, b_col, b_score, top_n, out_indptr, out_row, out_col, out_score, big_rows, n_big);
+        SG_LAUNCH_CHECK();
+    } else {
+        sel_rows_small_kernel<false><<<(unsigned)((n_rows + 7) / 8), 256, 0, st>>>(
+            n_rows, row_begin, row_start, b_col, b_score, top_n, out_indptr, out_row, out_col, out_score, big_rows, n_big);
+        SG_LAUNCH_CHECK();
+        int dev = 0, n_sm = 0;
+        SG_CUDA_TRY(cudaGetDevice(&dev));
+        SG_CUDA_TRY(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
+        sel_rows_mid_kernel<<<(unsigned)(n_sm * 2), SEL_MID_WARPS * 32, 0, st>>>(row_begin, row_start, b_col, b_score,
+                                                                                top_n, out_indptr, out_row, out_col,
+                                                                                out_score, big_rows, n_big);
+        SG_LAUNCH_CHECK();
+        sel_rows_big_kernel<<<(unsigned)(n_sm * 2), 256, 0, st>>>(row_begin, row_start, b_col, b_score, top_n, out_indptr,
+                                                                 out_row, out_col, out_score, big_rows, n_big);
+        SG_LAUNCH_CHECK();
+    }
+    return SG_OK;
+}
+
+// ---- the dedup path's selection (sg_topn_select_groups): kept pairs (u, v, s) of groups of bit-identical rows ----
+
+constexpr int GRP_INLINE = 16;           // members of v one thread writes itself; larger groups go to whole warps
+
+// survivors per group u once every kept (u, v) stands for the |v| columns of group v
+__global__ void grp_count_kernel(int64_t n, const int32_t *__restrict__ cr, const int32_t *__restrict__ cc,
+                                 const int32_t *__restrict__ mem_ptr, int32_t *__restrict__ grp_cnt) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int32_t v = cc[i];
+    atomicAdd(grp_cnt + cr[i], mem_ptr[v + 1] - mem_ptr[v]);
+}
+
+// totals[0] = expanded survivors, totals[1] = output pairs (every member of u gets min(count, top_n) of them)
+__global__ void grp_totals_kernel(int64_t m, const int32_t *__restrict__ grp_cnt, const int32_t *__restrict__ mem_ptr,
+                                  int top_n, unsigned long long *__restrict__ totals) {
+    const int64_t u = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    unsigned long long e = 0, o = 0;
+    if (u < m) {
+        const int c = grp_cnt[u];
+        e = (unsigned long long)c;
+        o = (unsigned long long)(mem_ptr[u + 1] - mem_ptr[u]) * (unsigned long long)(c < top_n ? c : top_n);
+    }
+#pragma unroll
+    for (int s = 16; s; s >>= 1) {
+        e += __shfl_xor_sync(FULL, e, s);
+        o += __shfl_xor_sync(FULL, o, s);
+    }
+    if (lane_id() == 0 && e) {
+        atomicAdd(totals, e);
+        atomicAdd(totals + 1, o);
+    }
+}
+
+// every kept (u, v, s) -> u's bucket once per member of v, with the member's row id as the column; groups of more
+// than GRP_INLINE members are left to grp_scatter_wide_kernel (one warp each), so no thread writes more than that
+__global__ void grp_scatter_kernel(int64_t n, const int32_t *__restrict__ cr, const int32_t *__restrict__ cc,
+                                   const double *__restrict__ score, const int32_t *__restrict__ mem_ptr,
+                                   const int32_t *__restrict__ mem_rows, const int64_t *__restrict__ row_start,
+                                   int32_t *__restrict__ fill, int32_t *__restrict__ b_col,
+                                   double *__restrict__ b_score, int32_t *__restrict__ wide,
+                                   int64_t *__restrict__ wide_pos, int32_t *__restrict__ n_wide) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int32_t u = cr[i], v = cc[i];
+    const int32_t m0 = mem_ptr[v], len = mem_ptr[v + 1] - m0;
+    const int64_t p = row_start[u] + atomicAdd(fill + u, len);
+    if (len > GRP_INLINE) {
+        const int32_t w = atomicAdd(n_wide, 1);
+        wide[w] = (int32_t)i;
+        wide_pos[w] = p;
+        return;
+    }
+    const double s = score[i];
+    for (int k = 0; k < len; ++k) {
+        b_col[p + k] = mem_rows[m0 + k];
+        b_score[p + k] = s;
+    }
+}
+
+__global__ void grp_scatter_wide_kernel(const int32_t *__restrict__ cc, const double *__restrict__ score,
+                                        const int32_t *__restrict__ mem_ptr, const int32_t *__restrict__ mem_rows,
+                                        const int32_t *__restrict__ wide, const int64_t *__restrict__ wide_pos,
+                                        const int32_t *__restrict__ n_wide, int32_t *__restrict__ b_col,
+                                        double *__restrict__ b_score) {
+    const int nw = *n_wide;
+    const int warps = gridDim.x * (blockDim.x >> 5);
+    for (int w = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); w < nw; w += warps) {
+        const int32_t i = wide[w], v = cc[i];
+        const int32_t m0 = mem_ptr[v], len = mem_ptr[v + 1] - m0;
+        const int64_t p = wide_pos[w];
+        const double s = score[i];
+        for (int k = lane_id(); k < len; k += 32) {
+            b_col[p + k] = mem_rows[m0 + k];
+            b_score[p + k] = s;
+        }
+    }
+}
+
+__global__ void grp_row_k_kernel(int64_t n_rows, const int32_t *__restrict__ uid, const int64_t *__restrict__ g_cnt,
+                                 int64_t *__restrict__ row_k) {
+    const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r < n_rows) row_k[r] = g_cnt[uid[r]];
+    else if (r == n_rows) row_k[r] = 0;
+}
+
+// one warp per row: its group's ranked list under the row's own id
+__global__ void grp_copy_kernel(int64_t n_rows, const int32_t *__restrict__ uid, const int64_t *__restrict__ g_indptr,
+                                const int32_t *__restrict__ g_col, const double *__restrict__ g_score,
+                                const int64_t *__restrict__ out_indptr, int32_t *__restrict__ out_row,
+                                int32_t *__restrict__ out_col, double *__restrict__ out_score) {
+    const int64_t r = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (r >= n_rows) return;
+    const int32_t u = uid[r];
+    const int64_t s = g_indptr[u], k = g_indptr[u + 1] - s, o = out_indptr[r];
+    for (int64_t j = lane_id(); j < k; j += 32) {
+        out_row[o + j] = (int32_t)r;
+        out_col[o + j] = g_col[s + j];
+        out_score[o + j] = g_score[s + j];
+    }
+}
+
+struct GroupsWs {
+    int32_t *b_col;
+    double *b_score;
+    int64_t *cnt64, *row_start, *out_cnt, *g_indptr;
+    int32_t *fill, *big_rows, *wide;
+    int64_t *wide_pos;
+    int32_t *g_row, *g_col;
+    double *g_score;
+    int64_t *row_k;
+    char *scan_tmp;
+    size_t scan_bytes;
+};
+
 }  // namespace sg
 
 using namespace sg;
@@ -353,26 +496,116 @@ int sg_topn_select_rows(int64_t n_cand, const int32_t *cand_row, const int32_t *
     sel_scatter_kernel<<<(unsigned)((n_cand + 255) / 256), 256, 0, st>>>(n_cand, cand_row, cand_col, score, row_begin,
                                                                         row_start, fill, b_col, b_score);
     SG_LAUNCH_CHECK();
-    if (top_n <= 32) {
-        // the common case (max_n_matches defaults to 20): every row, whatever its length, by one warp
-        sel_rows_small_kernel<true><<<(unsigned)((n_rows + 7) / 8), 256, 0, st>>>(
-            n_rows, row_begin, row_start, b_col, b_score, top_n, out_indptr, out_row, out_col, out_score, big_rows, n_big);
-        SG_LAUNCH_CHECK();
-    } else {
-        sel_rows_small_kernel<false><<<(unsigned)((n_rows + 7) / 8), 256, 0, st>>>(
-            n_rows, row_begin, row_start, b_col, b_score, top_n, out_indptr, out_row, out_col, out_score, big_rows, n_big);
-        SG_LAUNCH_CHECK();
-        int dev = 0, n_sm = 0;
-        SG_CUDA_TRY(cudaGetDevice(&dev));
-        SG_CUDA_TRY(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
-        sel_rows_mid_kernel<<<(unsigned)(n_sm * 2), SEL_MID_WARPS * 32, 0, st>>>(row_begin, row_start, b_col, b_score,
-                                                                                top_n, out_indptr, out_row, out_col,
-                                                                                out_score, big_rows, n_big);
-        SG_LAUNCH_CHECK();
-        sel_rows_big_kernel<<<(unsigned)(n_sm * 2), 256, 0, st>>>(row_begin, row_start, b_col, b_score, top_n, out_indptr,
-                                                                 out_row, out_col, out_score, big_rows, n_big);
+    const int rc = sel_rank_rows(n_rows, row_begin, row_start, b_col, b_score, top_n, out_indptr, out_row, out_col,
+                                 out_score, big_rows, n_big, st);
+    if (rc != SG_OK) return rc;
+    sel_finish_kernel<<<1, 32, 0, st>>>(n_rows, out_indptr, out_nnz);
+    SG_LAUNCH_CHECK();
+    return SG_OK;
+}
+
+int sg_topn_groups_count(int64_t n_cand, const int32_t *cand_row, const int32_t *cand_col, int64_t n_groups,
+                         const int32_t *mem_ptr, int top_n, int32_t *grp_cnt, int64_t *totals, void *stream_) {
+    cudaStream_t st = (cudaStream_t)stream_;
+    if (n_cand < 0 || n_groups < 0) return fail(SG_ERR_INVALID, "negative size");
+    SG_CUDA_TRY(cudaMemsetAsync(totals, 0, 2 * sizeof(int64_t), st));
+    if (n_groups == 0) return SG_OK;
+    SG_CUDA_TRY(cudaMemsetAsync(grp_cnt, 0, (size_t)n_groups * sizeof(int32_t), st));
+    if (n_cand > 0) {
+        grp_count_kernel<<<(unsigned)((n_cand + 255) / 256), 256, 0, st>>>(n_cand, cand_row, cand_col, mem_ptr, grp_cnt);
         SG_LAUNCH_CHECK();
     }
+    grp_totals_kernel<<<(unsigned)((n_groups + 255) / 256), 256, 0, st>>>(n_groups, grp_cnt, mem_ptr, top_n,
+                                                                         (unsigned long long *)totals);
+    SG_LAUNCH_CHECK();
+    return SG_OK;
+}
+
+static size_t groups_carve(Arena &ar, int64_t n_cand, int64_t n_expanded, int64_t n_groups, int64_t n_rows,
+                           int top_n, GroupsWs *w) {
+    GroupsWs d{};
+    const int64_t e = n_expanded < 1 ? 1 : n_expanded;
+    const int64_t c = n_cand < 1 ? 1 : n_cand;
+    int64_t g = n_groups * (int64_t)(top_n < 1 ? 1 : top_n);
+    g = g < e ? g : e;
+    const size_t m2 = (size_t)n_groups + 2;
+    d.b_col = ar.take<int32_t>((size_t)e);
+    d.b_score = ar.take<double>((size_t)e);
+    d.cnt64 = ar.take<int64_t>(m2);
+    d.row_start = ar.take<int64_t>(m2);
+    d.out_cnt = ar.take<int64_t>(m2);
+    d.g_indptr = ar.take<int64_t>(m2);
+    d.fill = ar.take<int32_t>(m2);
+    d.big_rows = ar.take<int32_t>(m2);
+    d.wide = ar.take<int32_t>((size_t)c);
+    d.wide_pos = ar.take<int64_t>((size_t)c);
+    d.g_row = ar.take<int32_t>((size_t)g);
+    d.g_col = ar.take<int32_t>((size_t)g);
+    d.g_score = ar.take<double>((size_t)g);
+    d.row_k = ar.take<int64_t>((size_t)n_rows + 2);
+    size_t a = 0, b = 0;
+    cub::DeviceScan::ExclusiveSum(nullptr, a, d.cnt64, d.row_start, n_groups + 1);
+    cub::DeviceScan::ExclusiveSum(nullptr, b, d.row_k, (int64_t *)nullptr, n_rows + 1);
+    d.scan_bytes = a > b ? a : b;
+    d.scan_tmp = ar.take<char>(d.scan_bytes);
+    if (w) *w = d;
+    return ar.off;
+}
+
+size_t sg_topn_select_groups_workspace_bytes(int64_t n_cand, int64_t n_expanded, int64_t n_groups, int64_t n_rows,
+                                             int top_n) {
+    Arena ar(nullptr, 0);
+    return groups_carve(ar, n_cand, n_expanded, n_groups, n_rows, top_n, nullptr) + 4096;
+}
+
+int sg_topn_select_groups(int64_t n_cand, const int32_t *cand_row, const int32_t *cand_col, const double *score,
+                          int64_t n_groups, const int32_t *mem_ptr, const int32_t *mem_rows, const int32_t *grp_cnt,
+                          int64_t n_expanded, int64_t n_rows, const int32_t *uid, int top_n, int64_t *out_indptr,
+                          int32_t *out_row, int32_t *out_col, double *out_score, int64_t *out_nnz,
+                          int32_t *out_max_row, void *ws, size_t ws_bytes, void *stream_) {
+    cudaStream_t st = (cudaStream_t)stream_;
+    if (n_rows < 0 || n_cand < 0 || n_groups < 0 || n_expanded < 0) return fail(SG_ERR_INVALID, "negative size");
+    SG_CUDA_TRY(cudaMemsetAsync(out_max_row, 0, sizeof(int32_t), st));
+    if (n_cand == 0 || top_n <= 0 || n_rows == 0 || n_groups == 0) {
+        SG_CUDA_TRY(cudaMemsetAsync(out_indptr, 0, (size_t)(n_rows + 1) * sizeof(int64_t), st));
+        SG_CUDA_TRY(cudaMemsetAsync(out_nnz, 0, sizeof(int64_t), st));
+        return SG_OK;
+    }
+    Arena ar(ws, ws_bytes);
+    GroupsWs w;
+    groups_carve(ar, n_cand, n_expanded, n_groups, n_rows, top_n, &w);
+    if (!ar.ok()) return fail(SG_ERR_INVALID, "select workspace too small (%zu < %zu)", ws_bytes, ar.off);
+    const int64_t m = n_groups;
+    int32_t *n_big = w.fill + m + 1;
+    int32_t *n_wide = w.big_rows + m + 1;
+    SG_CUDA_TRY(cudaMemsetAsync(w.fill, 0, (size_t)(m + 2) * sizeof(int32_t), st));
+    SG_CUDA_TRY(cudaMemsetAsync(n_wide, 0, sizeof(int32_t), st));
+    // group space: survivors (expanded) per group, the group lists' offsets, the largest list (= the largest row's)
+    sel_counts_kernel<<<(unsigned)((m + 1 + 255) / 256), 256, 0, st>>>(m, grp_cnt, top_n, w.cnt64, w.out_cnt,
+                                                                      out_max_row);
+    SG_LAUNCH_CHECK();
+    SG_CUDA_TRY(cub::DeviceScan::ExclusiveSum(w.scan_tmp, w.scan_bytes, w.cnt64, w.row_start, m + 1, st));
+    SG_CUDA_TRY(cub::DeviceScan::ExclusiveSum(w.scan_tmp, w.scan_bytes, w.out_cnt, w.g_indptr, m + 1, st));
+    grp_scatter_kernel<<<(unsigned)((n_cand + 255) / 256), 256, 0, st>>>(n_cand, cand_row, cand_col, score, mem_ptr,
+                                                                        mem_rows, w.row_start, w.fill, w.b_col,
+                                                                        w.b_score, w.wide, w.wide_pos, n_wide);
+    SG_LAUNCH_CHECK();
+    int dev = 0, n_sm = 0;
+    SG_CUDA_TRY(cudaGetDevice(&dev));
+    SG_CUDA_TRY(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
+    grp_scatter_wide_kernel<<<(unsigned)(n_sm * 8), 256, 0, st>>>(cand_col, score, mem_ptr, mem_rows, w.wide,
+                                                                  w.wide_pos, n_wide, w.b_col, w.b_score);
+    SG_LAUNCH_CHECK();
+    const int rc = sel_rank_rows(m, 0, w.row_start, w.b_col, w.b_score, top_n, w.g_indptr, w.g_row, w.g_col,
+                                 w.g_score, w.big_rows, n_big, st);
+    if (rc != SG_OK) return rc;
+    // every row: a copy of its group's list
+    grp_row_k_kernel<<<(unsigned)((n_rows + 1 + 255) / 256), 256, 0, st>>>(n_rows, uid, w.out_cnt, w.row_k);
+    SG_LAUNCH_CHECK();
+    SG_CUDA_TRY(cub::DeviceScan::ExclusiveSum(w.scan_tmp, w.scan_bytes, w.row_k, out_indptr, n_rows + 1, st));
+    grp_copy_kernel<<<(unsigned)((n_rows + 7) / 8), 256, 0, st>>>(n_rows, uid, w.g_indptr, w.g_col, w.g_score,
+                                                                  out_indptr, out_row, out_col, out_score);
+    SG_LAUNCH_CHECK();
     sel_finish_kernel<<<1, 32, 0, st>>>(n_rows, out_indptr, out_nnz);
     SG_LAUNCH_CHECK();
     return SG_OK;
