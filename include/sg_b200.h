@@ -136,6 +136,45 @@ int sg_tfidf64_values(const int64_t *offsets /*[dev]*/, int64_t n_docs, int dtyp
                       double *val64 /*[dev] total or NULL*/, float *val32 /*[dev] total*/, void *stream);
 
 /* ------------------------------------------------------------------------- *
+ * K1 transform: new documents through a FITTED vocabulary (TfidfVectorizer.transform).  N-grams outside the
+ * vocabulary are dropped, tf counts the known ones, idf and columns are the fitted ones, the L2 norm is taken after
+ * the drop; a row without a known n-gram is empty.  The fitted vocabulary is only read.
+ *
+ * Dense form (ASCII, ngram <= 3 vocabulary of sg_tfidf_vocab):
+ *   sg_tfidf_transform_count  = sg_tfidf_count without the df update;
+ *   sg_tfidf_known            keeps the runs whose key has df_table[key] > 0 (compacted in place, row_nnz := kept),
+ *                             indptr = exclusive scan;
+ *   sg_tfidf_values           with the fitted rank_table and idf.
+ * Sorted form (vocabulary of sg_tfidf64_vocab, or any vocabulary given as its sorted keys):
+ *   sg_tfidf64_transform_count = sg_tfidf64_count over symbols mapped through the FITTED alphabet; a symbol outside
+ *                             it is SG_SYMBOL_UNKNOWN (sym_width 4) or SG_LUT_UNKNOWN in the byte table, and no
+ *                             n-gram containing it is emitted (no neighbouring id can alias a real key);
+ *   sg_tfidf64_known          binary search of every run's key in vocab_keys[V] (sorted ascending), unknown runs
+ *                             dropped, indptr, indices; scratch_col has total entries;
+ *   sg_tfidf64_values         with the fitted idf.
+ * Workspace of both *_known: sg_tfidf_transform_workspace_bytes(n_docs).
+ * ------------------------------------------------------------------------- */
+#define SG_SYMBOL_UNKNOWN 0xffffffffu
+#define SG_LUT_UNKNOWN 0xfeu
+int sg_tfidf_transform_count(const uint8_t *bytes /*[dev]*/, const int64_t *offsets /*[dev] n_docs+1*/,
+                             int64_t n_docs, int ngram, unsigned flags, uint8_t *scratch_clean /*[dev]*/,
+                             uint32_t *scratch_sort /*[dev]*/, uint32_t *scratch_key /*[dev]*/,
+                             uint32_t *scratch_tf /*[dev]*/, int32_t *row_nnz /*[dev] n_docs+1*/, void *stream);
+size_t sg_tfidf_transform_workspace_bytes(int64_t n_docs);
+int sg_tfidf_known(const int64_t *offsets /*[dev]*/, int64_t n_docs, const int32_t *df_table /*[dev] slots*/,
+                   uint32_t *scratch_key /*[dev]*/, uint32_t *scratch_tf /*[dev]*/, int32_t *row_nnz /*[dev] n_docs+1*/,
+                   int64_t *indptr /*[dev] n_docs+1*/, void *ws /*[dev]*/, size_t ws_bytes, void *stream);
+int sg_tfidf64_transform_count(const void *symbols /*[dev]*/, int sym_width, const int64_t *offsets /*[dev]*/,
+                               int64_t n_docs, int ngram, int bits, const uint8_t *lut /*[dev] 256 or NULL*/,
+                               uint32_t *scratch_clean, uint64_t *scratch_sort, uint64_t *scratch_key,
+                               uint32_t *scratch_tf, int32_t *row_nnz /*[dev] n_docs+1*/, void *stream);
+int sg_tfidf64_known(const int64_t *offsets /*[dev]*/, int64_t n_docs, const uint64_t *vocab_keys /*[dev] V*/,
+                     int32_t vocab_size, const uint64_t *scratch_key /*[dev]*/, uint32_t *scratch_tf /*[dev]*/,
+                     int32_t *scratch_col /*[dev] total*/, int32_t *row_nnz /*[dev] n_docs+1*/,
+                     int64_t *indptr /*[dev] n_docs+1*/, int32_t *indices /*[dev] total*/, void *ws /*[dev]*/,
+                     size_t ws_bytes, void *stream);
+
+/* ------------------------------------------------------------------------- *
  * K2 — blocked CSR x CSR^T, thresholded, top-n per left row.
  * Replaces: StringGrouper._build_matches (sg.py:709-752), i.e. the
  * sp_matmul_topn block products (:737-743), the zip over right blocks (:746)

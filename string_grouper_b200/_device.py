@@ -1448,12 +1448,28 @@ def _upload_idf(df_host, n_docs_fit, np_dtype, device):
 
 class DeviceVocabulary:
     """df / rank tables of the fitted vectoriser (the device twin of TfidfVectorizer.vocabulary_); `idf_` is the
-    twin of TfidfVectorizer.idf_ (numpy, matrix dtype)."""
+    twin of TfidfVectorizer.idf_ (numpy, matrix dtype), `d_idf` its device copy."""
 
-    def __init__(self, df_table, rank_table, ngram, n_docs, vocab_size, idf=None):
+    # as a sorted vocabulary (tfidf_transform of code points): the packed keys are n-grams over the 128 ASCII codes
+    alphabet = np.arange(128, dtype=np.uint32)
+    bits = 7
+
+    def __init__(self, df_table, rank_table, ngram, n_docs, vocab_size, idf=None, d_idf=None):
         self.d_df, self.d_rank = df_table, rank_table
         self.ngram, self.n_docs, self.size = int(ngram), int(n_docs), int(vocab_size)
-        self.idf_ = idf
+        self.idf_, self.d_idf = idf, d_idf
+        self._sorted_keys = None
+
+    def sorted_keys(self):
+        """int64 packed key of every column, ascending (cached)."""
+        if self._sorted_keys is None:
+            t = require_cuda()
+            L = _lib.load()
+            keys = _empty(self.size, t.int32, self.d_df.device)
+            _lib.check(L.sg_tfidf_vocab_keys(_ptr(self.d_df), _ptr(self.d_rank), self.ngram, _ptr(keys), _stream()))
+            self._sorted_keys = keys.to(t.int64)
+            LAUNCH_COUNTS["tfidf"] += 1
+        return self._sorted_keys
 
     def feature_names(self):
         """Sorted n-grams, column order of the TF-IDF matrices (sklearn get_feature_names_out)."""
@@ -1479,10 +1495,14 @@ def upload_strings(data, offsets, device=None):
 class DeviceVocabulary64:
     """Sorted vocabulary of the general vectoriser (csrc/sg_tfidf64.cu): 64-bit keys over a dense alphabet."""
 
-    def __init__(self, keys, df, alphabet, bits, ngram, n_docs, vocab_size, idf=None):
+    def __init__(self, keys, df, alphabet, bits, ngram, n_docs, vocab_size, idf=None, d_idf=None):
         self.d_keys, self.d_df, self.alphabet = keys, df, alphabet
         self.bits, self.ngram, self.n_docs, self.size = int(bits), int(ngram), int(n_docs), int(vocab_size)
-        self.idf_ = idf
+        self.idf_, self.d_idf = idf, d_idf
+
+    def sorted_keys(self):
+        """int64 (bit pattern of uint64) key of every column, ascending."""
+        return self.d_keys
 
     def feature_names(self):
         from ._ingest import decode_vocab_keys64
@@ -1553,7 +1573,7 @@ def tfidf_sorted(data, offsets, n_master, ngram, flags, dtype, device=None, stat
                                    _ptr(val64), _ptr(val32), _stream()))
     LAUNCH_COUNTS["tfidf"] += 7
     val = val64 if np_dtype == np.float64 else val32
-    vocab = DeviceVocabulary64(vocab_keys, df, alphabet, bits, ngram, n_docs, V, idf)
+    vocab = DeviceVocabulary64(vocab_keys, df, alphabet, bits, ngram, n_docs, V, idf, d_idf)
     if stats is not None:
         stats.update(n_docs=n_docs, total_bytes=total, nnz=nnz, vocab=V, h2d_bytes=int(total * sym_width + 8 * len(offsets)),
                      vectoriser="sorted vocabulary, %d-bit keys" % (int(ngram) * bits))
@@ -1637,7 +1657,7 @@ def tfidf_resident(d_bytes, d_off, n_docs, total, n_master, ngram, flags, dtype,
                                  _ptr(row_nnz), _ptr(indptr), _ptr(indices), _ptr(val64), _ptr(val32), _stream()))
     LAUNCH_COUNTS["tfidf"] += 5
     val = val64 if np_dtype == np.float64 else val32
-    vocab = DeviceVocabulary(df, rank, ngram, n_fit, V, idf)
+    vocab = DeviceVocabulary(df, rank, ngram, n_fit, V, idf, d_idf)
     if stats is not None:
         stats.update(n_docs=n_docs, total_bytes=total, nnz=nnz, vocab=V)
     master = DeviceCSR((n_master, V), indptr[:n_master + 1], indices, val, val32, split, np_dtype, 1.0, base=0)
@@ -1651,6 +1671,88 @@ def tfidf_resident(d_bytes, d_off, n_docs, total, n_master, ngram, flags, dtype,
                     base=split)
     dup.nnz_parent = nnz
     return master, dup, vocab
+
+
+def tfidf_transform(data, offsets, n_first, flags, vocab, stats=None):
+    """K1 transform: packed strings (as _ingest.pack_strings returns them) -> TF-IDF rows over the FITTED vocabulary
+    `vocab` (TfidfVectorizer.transform): n-grams outside it are dropped, tf counts the known ones, idf and columns are
+    the vocabulary's, the L2 norm is taken after the drop.  `vocab` is only read.  Returns (rows [0, n_first), rows
+    [n_first, n_docs)) as DeviceCSR views of the same arrays.
+
+    ASCII bytes against a dense vocabulary (ngram_size <= 3) take the dense form (key table lookup); everything else
+    the sorted form: symbols mapped through the vocabulary's alphabet (an ASCII vocabulary's is the 128 codes of its
+    7-bit keys), keys found by binary search among its sorted keys."""
+    t = require_cuda()
+    L = _lib.load()
+    from . import _ingest
+    device = vocab.d_idf.device
+    n_docs = len(offsets) - 1
+    total = int(offsets[-1])
+    np_dtype = np.dtype(vocab.idf_.dtype)
+    dt = _lib.SG_DTYPE_F32 if np_dtype == np.float32 else _lib.SG_DTYPE_F64
+    V = vocab.size
+    row_nnz = _empty(n_docs + 1, t.int32, device)
+    indptr = _empty(n_docs + 1, t.int64, device)
+    indices = _empty(total, t.int32, device)
+    val32 = _empty(total, t.float32, device)
+    val64 = _empty(total, t.float64, device) if np_dtype == np.float64 else None
+    ws_bytes = int(L.sg_tfidf_transform_workspace_bytes(n_docs))
+    ws = _empty(ws_bytes, t.uint8, device)
+    if isinstance(vocab, DeviceVocabulary) and data.dtype == np.uint8:
+        d_bytes, d_off, _ = upload_strings(data, offsets, device)
+        h2d = int(total + 8 * len(offsets))
+        s_clean = _empty(total, t.uint8, device)
+        s_sort = _empty(total, t.int32, device)
+        s_key = _empty(total, t.int32, device)
+        s_tf = _empty(total, t.int32, device)
+        _lib.check(L.sg_tfidf_transform_count(_ptr(d_bytes), _ptr(d_off), n_docs, vocab.ngram, int(flags),
+                                              _ptr(s_clean), _ptr(s_sort), _ptr(s_key), _ptr(s_tf), _ptr(row_nnz),
+                                              _stream()))
+        _lib.check(L.sg_tfidf_known(_ptr(d_off), n_docs, _ptr(vocab.d_df), _ptr(s_key), _ptr(s_tf), _ptr(row_nnz),
+                                    _ptr(indptr), _ptr(ws), ws_bytes, _stream()))
+        _lib.check(L.sg_tfidf_values(_ptr(d_off), n_docs, dt, _ptr(vocab.d_idf), _ptr(vocab.d_rank), _ptr(s_key),
+                                     _ptr(s_tf), _ptr(row_nnz), _ptr(indptr), _ptr(indices), _ptr(val64), _ptr(val32),
+                                     _stream()))
+        LAUNCH_COUNTS["tfidf"] += 3
+        form = "dense key table"
+    else:
+        keys = vocab.sorted_keys()
+        if data.dtype == np.uint8:
+            sym_width = 1
+            d_sym = t.from_numpy(np.ascontiguousarray(data)).to(device) if total else _empty(1, t.uint8, device)
+            d_lut = t.from_numpy(_ingest.fitted_byte_lut(data, flags, vocab.alphabet)).to(device)
+        else:
+            sym_width = 4
+            ids = _ingest.fitted_symbol_ids(data, vocab.alphabet)
+            d_sym = t.from_numpy(ids.view(np.int32)).to(device) if total else _empty(1, t.int32, device)
+            d_lut = None
+        d_off = t.from_numpy(np.ascontiguousarray(offsets, dtype=np.int64)).to(device)
+        h2d = int(total * sym_width + 8 * len(offsets))
+        s_clean = _empty(total, t.int32, device)
+        s_sort = _empty(total, t.int64, device)
+        s_key = _empty(total, t.int64, device)
+        s_tf = _empty(total, t.int32, device)
+        s_col = _empty(total, t.int32, device)
+        _lib.check(L.sg_tfidf64_transform_count(_ptr(d_sym), sym_width, _ptr(d_off), n_docs, vocab.ngram, vocab.bits,
+                                                _ptr(d_lut), _ptr(s_clean), _ptr(s_sort), _ptr(s_key), _ptr(s_tf),
+                                                _ptr(row_nnz), _stream()))
+        _lib.check(L.sg_tfidf64_known(_ptr(d_off), n_docs, _ptr(keys), V, _ptr(s_key), _ptr(s_tf), _ptr(s_col),
+                                      _ptr(row_nnz), _ptr(indptr), _ptr(indices), _ptr(ws), ws_bytes, _stream()))
+        _lib.check(L.sg_tfidf64_values(_ptr(d_off), n_docs, dt, _ptr(vocab.d_idf), _ptr(s_tf), _ptr(indptr),
+                                       _ptr(indices), _ptr(val64), _ptr(val32), _stream()))
+        LAUNCH_COUNTS["tfidf"] += 4
+        form = "sorted vocabulary, %d-bit keys" % (vocab.ngram * vocab.bits)
+    TRANSFER_BYTES["h2d"] += h2d
+    n_first = int(n_first)
+    split, nnz = (int(x) for x in t.cat([indptr[n_first:n_first + 1], indptr[n_docs:n_docs + 1]]).cpu().numpy())
+    if stats is not None:
+        stats.update(n_docs=n_docs, total_bytes=total, nnz=nnz, vocab=V, h2d_bytes=h2d, vectoriser="transform, " + form)
+    val = val64 if np_dtype == np.float64 else val32
+    first = DeviceCSR((n_first, V), indptr[:n_first + 1], indices, val, val32, split, np_dtype, 1.0, base=0)
+    second = DeviceCSR((n_docs - n_first, V), indptr[n_first:], indices, val, val32, nnz - split, np_dtype, 1.0,
+                       base=split)
+    first.nnz_parent = second.nnz_parent = nnz
+    return first, second
 
 
 def as_device_matches(m):

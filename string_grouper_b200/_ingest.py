@@ -19,7 +19,7 @@ import numpy as np
 import pandas as pd
 import pyarrow as pa
 
-from ._lib import SG_FLAG_IGNORE_CASE, SG_FLAG_STRIP_DEFAULT
+from ._lib import SG_FLAG_IGNORE_CASE, SG_FLAG_STRIP_DEFAULT, SG_LUT_UNKNOWN, SG_SYMBOL_UNKNOWN
 
 DEFAULT_REGEX = r'[,-./]|\s'
 
@@ -191,9 +191,8 @@ def is_stripped(c):
     return (0x2c <= c <= 0x2f) or (0x09 <= c <= 0x0d) or (0x1c <= c <= 0x20)
 
 
-def byte_alphabet(data, flags):
-    """Dense, order-preserving alphabet of the bytes that survive folding / stripping: (lut uint8[256] with 0xff =
-    deleted, alphabet = array of the surviving code points in ascending order)."""
+def _byte_symbols(data, flags):
+    """{byte present in `data`: its character after case folding} for the bytes the default regex does not delete"""
     hist = np.bincount(data, minlength=256) if data.size else np.zeros(256, dtype=np.int64)
     fold, strip = bool(flags & SG_FLAG_IGNORE_CASE), bool(flags & SG_FLAG_STRIP_DEFAULT)
     mapped = {}
@@ -202,12 +201,40 @@ def byte_alphabet(data, flags):
         if strip and is_stripped(c2):
             continue
         mapped[c] = c2
+    return mapped
+
+
+def byte_alphabet(data, flags):
+    """Dense, order-preserving alphabet of the bytes that survive folding / stripping: (lut uint8[256] with 0xff =
+    deleted, alphabet = array of the surviving code points in ascending order)."""
+    mapped = _byte_symbols(data, flags)
     alphabet = np.array(sorted(set(mapped.values())), dtype=np.uint32)
     ids = {int(c): i for i, c in enumerate(alphabet.tolist())}
     lut = np.full(256, 0xff, dtype=np.uint8)
     for c, c2 in mapped.items():
         lut[c] = ids[c2]
     return lut, alphabet
+
+
+def fitted_byte_lut(data, flags, alphabet):
+    """lut uint8[256] of new bytes through a FITTED alphabet (K1 transform): the symbol id of the folded byte, 0xff =
+    deleted, SG_LUT_UNKNOWN = a character the fitted alphabet does not hold."""
+    lut = np.full(256, 0xff, dtype=np.uint8)
+    for c, c2 in _byte_symbols(data, flags).items():
+        i = int(np.searchsorted(alphabet, c2))
+        lut[c] = i if i < len(alphabet) and int(alphabet[i]) == c2 else SG_LUT_UNKNOWN
+    return lut
+
+
+def fitted_symbol_ids(code_points, alphabet):
+    """uint32 symbol ids of new code points through a FITTED alphabet (K1 transform); SG_SYMBOL_UNKNOWN where the
+    alphabet does not hold the character (no nearest id: it would alias a real n-gram)."""
+    code_points = np.asarray(code_points, dtype=np.uint32)
+    if not len(alphabet):
+        return np.full(len(code_points), SG_SYMBOL_UNKNOWN, dtype=np.uint32)
+    ids = np.searchsorted(alphabet, code_points)
+    found = alphabet[np.minimum(ids, len(alphabet) - 1)] == code_points
+    return np.where(found, ids, SG_SYMBOL_UNKNOWN).astype(np.uint32)
 
 
 def symbol_bits(n_symbols):

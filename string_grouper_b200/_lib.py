@@ -25,6 +25,8 @@ SG_ACC_F32 = 0
 SG_ACC_U16 = 1
 SG_FLOOR_SEED = 1
 SG_FLOOR_LONG_ROWS = 2
+SG_SYMBOL_UNKNOWN = 0xffffffff      # a query symbol outside the fitted alphabet (K1 transform)
+SG_LUT_UNKNOWN = 0xfe
 
 _i64 = ctypes.c_int64
 _i32 = ctypes.c_int
@@ -50,6 +52,11 @@ SIGNATURES = {
     "sg_tfidf64_vocab_workspace_bytes": (_sz, [_i64, _i64]),
     "sg_tfidf64_vocab": (_i32, [_p, _i64, _i64, _i32, _i32, _p, _p, _p, _p, _p, _p, _p, _p, _p, _sz, _p]),
     "sg_tfidf64_values": (_i32, [_p, _i64, _i32, _p, _p, _p, _p, _p, _p, _p]),
+    "sg_tfidf_transform_count": (_i32, [_p, _p, _i64, _i32, _u32, _p, _p, _p, _p, _p, _p]),
+    "sg_tfidf_transform_workspace_bytes": (_sz, [_i64]),
+    "sg_tfidf_known": (_i32, [_p, _i64, _p, _p, _p, _p, _p, _p, _sz, _p]),
+    "sg_tfidf64_transform_count": (_i32, [_p, _i32, _p, _i64, _i32, _i32, _p, _p, _p, _p, _p, _p, _p]),
+    "sg_tfidf64_known": (_i32, [_p, _i64, _p, _i32, _p, _p, _p, _p, _p, _p, _p, _sz, _p]),
     "sg_num_tiles": (_i64, [_i64, _i32]),
     "sg_num_tiles_padded": (_i64, [_i64, _i32]),
     "sg_postings_workspace_bytes": (_sz, [_i64, _i64, _i64]),

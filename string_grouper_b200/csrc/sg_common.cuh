@@ -52,4 +52,8 @@ constexpr float FLOOR_EPS = 1e-6f;
 
 __device__ __forceinline__ int lane_id() { return threadIdx.x & 31; }
 
+// K1 transform (sg_tfidf.cu): indptr = exclusive scan of the kept runs per row (row_nnz, n_docs + 1 slots; the last is
+// zeroed here), workspace of sg_tfidf_transform_workspace_bytes
+int transform_indptr(int64_t n_docs, int32_t *row_nnz, int64_t *indptr, void *ws, size_t ws_bytes, cudaStream_t st);
+
 }  // namespace sg

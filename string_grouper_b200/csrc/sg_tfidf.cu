@@ -63,7 +63,9 @@ __device__ void warp_sort_keys(uint32_t *keys, int G, int lane) {
     }
 }
 
-// Run-length encode the sorted keys into (out_key, out_tf); one df increment per run.
+// Run-length encode the sorted keys into (out_key, out_tf); one df increment per run when kDf (a fit; a transform
+// through a fitted vocabulary leaves its df table alone).
+template <bool kDf>
 __device__ int warp_unique_count(const uint32_t *keys, int G, uint32_t *out_key, uint32_t *out_tf,
                                  int32_t *df, int lane) {
     int nheads = 0;
@@ -86,7 +88,7 @@ __device__ int warp_unique_count(const uint32_t *keys, int G, uint32_t *out_key,
             const int h = nheads + __popc(hb & ((1u << lane) - 1u));
             out_key[h] = k;
             out_tf[h] = (uint32_t)cnt;
-            atomicAdd(df + k, 1);
+            if (kDf) atomicAdd(df + k, 1);
         }
         nheads += __popc(hb);
         __syncwarp();
@@ -94,6 +96,7 @@ __device__ int warp_unique_count(const uint32_t *keys, int G, uint32_t *out_key,
     return nheads;
 }
 
+template <bool kDf>
 __global__ void __launch_bounds__(K1_WARPS * 32)
 tfidf_count_kernel(const uint8_t *__restrict__ bytes, const int64_t *__restrict__ offsets, int64_t n_docs,
                    int ngram, unsigned flags, int32_t *__restrict__ df, uint8_t *__restrict__ scratch_clean,
@@ -129,9 +132,42 @@ tfidf_count_kernel(const uint8_t *__restrict__ bytes, const int64_t *__restrict_
         }
         __syncwarp();
         warp_sort_keys(keys, G, lane);
-        const int nnz = warp_unique_count(keys, G, scratch_key + s, scratch_tf + s, df, lane);
+        const int nnz = warp_unique_count<kDf>(keys, G, scratch_key + s, scratch_tf + s, df, lane);
         if (lane == 0) row_nnz[doc] = nnz;
         __syncwarp();
+    }
+}
+
+// Transform: keep the (key, tf) runs of a document whose key the fitted vocabulary holds (df > 0), compacted in place
+// at the front of the document's scratch.  Keys stay ascending, so the kept runs are in column order.
+__global__ void __launch_bounds__(K1_WARPS * 32)
+tfidf_known_kernel(const int64_t *__restrict__ offsets, int64_t n_docs, const int32_t *__restrict__ df,
+                   uint32_t *__restrict__ scratch_key, uint32_t *__restrict__ scratch_tf, int32_t *__restrict__ row_nnz) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (int64_t doc = (int64_t)blockIdx.x * K1_WARPS + warp; doc < n_docs; doc += (int64_t)gridDim.x * K1_WARPS) {
+        const int64_t s = offsets[doc];
+        const int nnz = row_nnz[doc];
+        int kept = 0;
+        for (int base = 0; base < nnz; base += 32) {
+            const int i = base + lane;
+            uint32_t key = 0, tf = 0;
+            bool keep = false;
+            if (i < nnz) {
+                key = scratch_key[s + i];
+                tf = scratch_tf[s + i];
+                keep = df[key] > 0;
+            }
+            // every lane has read its run before any writes: the writes land at or before the positions read
+            const unsigned kb = __ballot_sync(FULL, keep);
+            if (keep) {
+                const int h = kept + __popc(kb & ((1u << lane) - 1u));
+                scratch_key[s + h] = key;
+                scratch_tf[s + h] = tf;
+            }
+            kept += __popc(kb);
+            __syncwarp();
+        }
+        if (lane == 0) row_nnz[doc] = kept;
     }
 }
 
@@ -211,6 +247,46 @@ __global__ void vocab_df_kernel(int64_t slots, const int32_t *__restrict__ df, c
     if (i < slots && df[i] > 0) df_out[rank[i]] = df[i];
 }
 
+// one warp per document, 8 resident CTAs of 8 warps per SM, grid-stride beyond
+static int k1_grid(int64_t n_docs, unsigned *grid_out) {
+    int dev = 0, n_sm = 0;
+    SG_CUDA_TRY(cudaGetDevice(&dev));
+    SG_CUDA_TRY(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
+    int64_t grid = (n_docs + K1_WARPS - 1) / K1_WARPS;
+    const int64_t cap = (int64_t)n_sm * 8;
+    *grid_out = (unsigned)(grid > cap ? cap : grid);
+    return SG_OK;
+}
+
+template <bool kDf>
+static int launch_count(const uint8_t *bytes, const int64_t *offsets, int64_t n_docs, int ngram, unsigned flags,
+                        int32_t *df_table, uint8_t *scratch_clean, uint32_t *scratch_sort, uint32_t *scratch_key,
+                        uint32_t *scratch_tf, int32_t *row_nnz, cudaStream_t st) {
+    if (ngram < 1 || ngram > 4)
+        return fail(SG_ERR_UNSUPPORTED, "ngram_size %d: the device vectoriser packs 7-bit characters into 32-bit keys "
+                                        "and supports 1 <= ngram_size <= 4", ngram);
+    if (n_docs <= 0) return SG_OK;
+    unsigned grid = 0;
+    const int rc = k1_grid(n_docs, &grid);
+    if (rc != SG_OK) return rc;
+    tfidf_count_kernel<kDf><<<grid, K1_WARPS * 32, 0, st>>>(bytes, offsets, n_docs, ngram, flags, df_table,
+                                                            scratch_clean, scratch_sort, scratch_key, scratch_tf,
+                                                            row_nnz);
+    SG_LAUNCH_CHECK();
+    return SG_OK;
+}
+
+int transform_indptr(int64_t n_docs, int32_t *row_nnz, int64_t *indptr, void *ws, size_t ws_bytes, cudaStream_t st) {
+    size_t b = 0;
+    cub::DeviceScan::ExclusiveScan(nullptr, b, (int32_t *)nullptr, (int64_t *)nullptr, cub::Sum(), (int64_t)0,
+                                   n_docs + 1);
+    if (ws_bytes < b) return fail(SG_ERR_INVALID, "tfidf transform workspace too small (%zu < %zu)", ws_bytes, b);
+    // row_nnz has n_docs+1 slots; the last one is a zero so that the scan yields indptr[n_docs]
+    SG_CUDA_TRY(cudaMemsetAsync(row_nnz + n_docs, 0, sizeof(int32_t), st));
+    SG_CUDA_TRY(cub::DeviceScan::ExclusiveScan(ws, b, row_nnz, indptr, cub::Sum(), (int64_t)0, n_docs + 1, st));
+    return SG_OK;
+}
+
 }  // namespace sg
 
 using namespace sg;
@@ -222,22 +298,38 @@ int64_t sg_tfidf_table_slots(int ngram) { return (ngram >= 1 && ngram <= 4) ? ((
 int sg_tfidf_count(const uint8_t *bytes, const int64_t *offsets, int64_t n_docs, int ngram, unsigned flags,
                    int32_t *df_table, uint8_t *scratch_clean, uint32_t *scratch_sort, uint32_t *scratch_key,
                    uint32_t *scratch_tf, int32_t *row_nnz, void *stream_) {
+    return launch_count<true>(bytes, offsets, n_docs, ngram, flags, df_table, scratch_clean, scratch_sort,
+                              scratch_key, scratch_tf, row_nnz, (cudaStream_t)stream_);
+}
+
+int sg_tfidf_transform_count(const uint8_t *bytes, const int64_t *offsets, int64_t n_docs, int ngram, unsigned flags,
+                             uint8_t *scratch_clean, uint32_t *scratch_sort, uint32_t *scratch_key,
+                             uint32_t *scratch_tf, int32_t *row_nnz, void *stream_) {
+    return launch_count<false>(bytes, offsets, n_docs, ngram, flags, nullptr, scratch_clean, scratch_sort,
+                               scratch_key, scratch_tf, row_nnz, (cudaStream_t)stream_);
+}
+
+size_t sg_tfidf_transform_workspace_bytes(int64_t n_docs) {
+    size_t b = 0;
+    cub::DeviceScan::ExclusiveScan(nullptr, b, (int32_t *)nullptr, (int64_t *)nullptr, cub::Sum(), (int64_t)0,
+                                   n_docs + 1);
+    return align_up(b, 256) + 256;
+}
+
+int sg_tfidf_known(const int64_t *offsets, int64_t n_docs, const int32_t *df_table, uint32_t *scratch_key,
+                   uint32_t *scratch_tf, int32_t *row_nnz, int64_t *indptr, void *ws, size_t ws_bytes,
+                   void *stream_) {
     cudaStream_t st = (cudaStream_t)stream_;
-    if (ngram < 1 || ngram > 4)
-        return fail(SG_ERR_UNSUPPORTED, "ngram_size %d: the device vectoriser packs 7-bit characters into 32-bit keys "
-                                        "and supports 1 <= ngram_size <= 4", ngram);
-    if (n_docs <= 0) return SG_OK;
-    int dev = 0, n_sm = 0;
-    SG_CUDA_TRY(cudaGetDevice(&dev));
-    SG_CUDA_TRY(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
-    int64_t grid = (n_docs + K1_WARPS - 1) / K1_WARPS;
-    const int64_t cap = (int64_t)n_sm * 8;   // 8 resident CTAs of 8 warps per SM, grid-stride beyond
-    if (grid > cap) grid = cap;
-    tfidf_count_kernel<<<(unsigned)grid, K1_WARPS * 32, 0, st>>>(bytes, offsets, n_docs, ngram, flags, df_table,
-                                                                 scratch_clean, scratch_sort, scratch_key,
-                                                                 scratch_tf, row_nnz);
-    SG_LAUNCH_CHECK();
-    return SG_OK;
+    if (n_docs < 0) return fail(SG_ERR_INVALID, "need n_docs >= 0");
+    if (n_docs > 0) {
+        unsigned grid = 0;
+        const int rc = k1_grid(n_docs, &grid);
+        if (rc != SG_OK) return rc;
+        tfidf_known_kernel<<<grid, K1_WARPS * 32, 0, st>>>(offsets, n_docs, df_table, scratch_key, scratch_tf,
+                                                           row_nnz);
+        SG_LAUNCH_CHECK();
+    }
+    return transform_indptr(n_docs, row_nnz, indptr, ws, ws_bytes, st);
 }
 
 size_t sg_tfidf_vocab_workspace_bytes(int64_t n_docs, int ngram) {

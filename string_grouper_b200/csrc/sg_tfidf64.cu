@@ -79,7 +79,9 @@ __device__ int warp_unique_count64(const uint64_t *keys, int G, uint64_t *out_ke
     return nheads;
 }
 
-template <typename SymT>
+// kTransform: the symbols were mapped through a fitted alphabet; a symbol outside it (SG_SYMBOL_UNKNOWN, or
+// SG_LUT_UNKNOWN from the byte table) has no id, so no n-gram containing it is emitted.
+template <typename SymT, bool kTransform>
 __global__ void __launch_bounds__(K64_WARPS * 32)
 tfidf64_count_kernel(const SymT *__restrict__ symbols, const int64_t *__restrict__ offsets, int64_t n_docs, int ngram,
                      int bits, const uint8_t *__restrict__ lut, uint32_t *__restrict__ scratch_clean,
@@ -108,6 +110,7 @@ tfidf64_count_kernel(const SymT *__restrict__ symbols, const int64_t *__restrict
                 if (sizeof(SymT) == 1) {
                     c = s_lut[(unsigned)symbols[s + i] & 0xffu];
                     keep = c != 0xffu;
+                    if (kTransform && c == SG_LUT_UNKNOWN) c = SG_SYMBOL_UNKNOWN;
                 } else {
                     c = (unsigned)symbols[s + i];
                     keep = true;
@@ -119,11 +122,30 @@ tfidf64_count_kernel(const SymT *__restrict__ symbols, const int64_t *__restrict
         }
         __syncwarp();
         const int64_t G64 = L - ngram + 1;
-        const int G = G64 > 0 ? (int)G64 : 0;
-        for (int j = lane; j < G; j += 32) {
-            uint64_t key = 0;
-            for (int q = 0; q < ngram; ++q) key = (key << bits) | (uint64_t)clean[j + q];
-            keys[j] = key;
+        int G = G64 > 0 ? (int)G64 : 0;
+        if (kTransform) {
+            // windows over an unknown symbol are dropped; the others are compacted in window order
+            int kept = 0;
+            for (int base = 0; base < G; base += 32) {
+                const int j = base + lane;
+                bool ok = j < G;
+                uint64_t key = 0;
+                for (int q = 0; ok && q < ngram; ++q) {
+                    const uint32_t c = clean[j + q];
+                    ok = c != SG_SYMBOL_UNKNOWN;
+                    key = (key << bits) | (uint64_t)c;
+                }
+                const unsigned kb = __ballot_sync(FULL, ok);
+                if (ok) keys[kept + __popc(kb & ((1u << lane) - 1u))] = key;
+                kept += __popc(kb);
+            }
+            G = kept;
+        } else {
+            for (int j = lane; j < G; j += 32) {
+                uint64_t key = 0;
+                for (int q = 0; q < ngram; ++q) key = (key << bits) | (uint64_t)clean[j + q];
+                keys[j] = key;
+            }
         }
         __syncwarp();
         warp_sort_keys64(keys, G, lane);
@@ -235,16 +257,61 @@ __global__ void tfidf64_tail_kernel(int64_t n_docs, const int64_t *__restrict__ 
     }
 }
 
-}  // namespace sg
+// Transform: the column of every (key, tf) run of a document by binary search in the fitted vocabulary's sorted keys;
+// runs whose key is not there are dropped, the others compacted in place (tf) and into scratch_col, in key order =
+// column order.
+__global__ void __launch_bounds__(K64_WARPS * 32)
+tfidf64_known_kernel(const int64_t *__restrict__ offsets, int64_t n_docs, const uint64_t *__restrict__ vocab_keys,
+                     int32_t vocab_size, const uint64_t *__restrict__ scratch_key, uint32_t *__restrict__ scratch_tf,
+                     int32_t *__restrict__ scratch_col, int32_t *__restrict__ row_nnz) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (int64_t doc = (int64_t)blockIdx.x * K64_WARPS + warp; doc < n_docs; doc += (int64_t)gridDim.x * K64_WARPS) {
+        const int64_t s = offsets[doc];
+        const int nnz = row_nnz[doc];
+        int kept = 0;
+        for (int base = 0; base < nnz; base += 32) {
+            const int i = base + lane;
+            int col = -1;
+            uint32_t tf = 0;
+            if (i < nnz) {
+                const uint64_t key = scratch_key[s + i];
+                tf = scratch_tf[s + i];
+                int lo = 0, hi = vocab_size;
+                while (lo < hi) {
+                    const int mid = (lo + hi) >> 1;
+                    if (vocab_keys[mid] < key) lo = mid + 1; else hi = mid;
+                }
+                if (lo < vocab_size && vocab_keys[lo] == key) col = lo;
+            }
+            // every lane has read its run before any writes: the writes land at or before the positions read
+            const unsigned kb = __ballot_sync(FULL, col >= 0);
+            if (col >= 0) {
+                const int h = kept + __popc(kb & ((1u << lane) - 1u));
+                scratch_tf[s + h] = tf;
+                scratch_col[s + h] = col;
+            }
+            kept += __popc(kb);
+            __syncwarp();
+        }
+        if (lane == 0) row_nnz[doc] = kept;
+    }
+}
 
-using namespace sg;
+// the kept columns from the documents' scratch positions to their CSR slots
+__global__ void tfidf64_place_kernel(int64_t n_docs, const int64_t *__restrict__ offsets,
+                                     const int64_t *__restrict__ indptr, const int32_t *__restrict__ scratch_col,
+                                     int32_t *__restrict__ indices) {
+    const int64_t doc = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (doc >= n_docs) return;
+    const int64_t s = offsets[doc], o = indptr[doc];
+    const int nnz = (int)(indptr[doc + 1] - o);
+    for (int i = lane_id(); i < nnz; i += 32) indices[o + i] = scratch_col[s + i];
+}
 
-extern "C" {
-
-int sg_tfidf64_count(const void *symbols, int sym_width, const int64_t *offsets, int64_t n_docs, int ngram, int bits,
-                     const uint8_t *lut, uint32_t *scratch_clean, uint64_t *scratch_sort, uint64_t *scratch_key,
-                     uint32_t *scratch_tf, int32_t *row_nnz, void *stream_) {
-    cudaStream_t st = (cudaStream_t)stream_;
+template <bool kTransform>
+static int launch_count64(const void *symbols, int sym_width, const int64_t *offsets, int64_t n_docs, int ngram,
+                          int bits, const uint8_t *lut, uint32_t *scratch_clean, uint64_t *scratch_sort,
+                          uint64_t *scratch_key, uint32_t *scratch_tf, int32_t *row_nnz, cudaStream_t st) {
     if (ngram < 1 || bits < 1 || (int64_t)ngram * bits > 64)
         return fail(SG_ERR_UNSUPPORTED, "ngram_size %d over %d-bit symbols needs %lld-bit keys (limit 64)", ngram, bits,
                     (long long)ngram * bits);
@@ -258,13 +325,55 @@ int sg_tfidf64_count(const void *symbols, int sym_width, const int64_t *offsets,
     const int64_t cap = (int64_t)n_sm * 6;
     if (grid > cap) grid = cap;
     if (sym_width == 1)
-        tfidf64_count_kernel<uint8_t><<<(unsigned)grid, K64_WARPS * 32, 0, st>>>(
+        tfidf64_count_kernel<uint8_t, kTransform><<<(unsigned)grid, K64_WARPS * 32, 0, st>>>(
             (const uint8_t *)symbols, offsets, n_docs, ngram, bits, lut, scratch_clean, scratch_sort, scratch_key,
             scratch_tf, row_nnz);
     else
-        tfidf64_count_kernel<uint32_t><<<(unsigned)grid, K64_WARPS * 32, 0, st>>>(
+        tfidf64_count_kernel<uint32_t, kTransform><<<(unsigned)grid, K64_WARPS * 32, 0, st>>>(
             (const uint32_t *)symbols, offsets, n_docs, ngram, bits, lut, scratch_clean, scratch_sort, scratch_key,
             scratch_tf, row_nnz);
+    SG_LAUNCH_CHECK();
+    return SG_OK;
+}
+
+}  // namespace sg
+
+using namespace sg;
+
+extern "C" {
+
+int sg_tfidf64_count(const void *symbols, int sym_width, const int64_t *offsets, int64_t n_docs, int ngram, int bits,
+                     const uint8_t *lut, uint32_t *scratch_clean, uint64_t *scratch_sort, uint64_t *scratch_key,
+                     uint32_t *scratch_tf, int32_t *row_nnz, void *stream_) {
+    return launch_count64<false>(symbols, sym_width, offsets, n_docs, ngram, bits, lut, scratch_clean, scratch_sort,
+                                 scratch_key, scratch_tf, row_nnz, (cudaStream_t)stream_);
+}
+
+int sg_tfidf64_transform_count(const void *symbols, int sym_width, const int64_t *offsets, int64_t n_docs, int ngram,
+                               int bits, const uint8_t *lut, uint32_t *scratch_clean, uint64_t *scratch_sort,
+                               uint64_t *scratch_key, uint32_t *scratch_tf, int32_t *row_nnz, void *stream_) {
+    return launch_count64<true>(symbols, sym_width, offsets, n_docs, ngram, bits, lut, scratch_clean, scratch_sort,
+                                scratch_key, scratch_tf, row_nnz, (cudaStream_t)stream_);
+}
+
+int sg_tfidf64_known(const int64_t *offsets, int64_t n_docs, const uint64_t *vocab_keys, int32_t vocab_size,
+                     const uint64_t *scratch_key, uint32_t *scratch_tf, int32_t *scratch_col, int32_t *row_nnz,
+                     int64_t *indptr, int32_t *indices, void *ws, size_t ws_bytes, void *stream_) {
+    cudaStream_t st = (cudaStream_t)stream_;
+    if (n_docs < 0 || vocab_size < 0) return fail(SG_ERR_INVALID, "need n_docs >= 0 and vocab_size >= 0");
+    if (n_docs == 0) return transform_indptr(n_docs, row_nnz, indptr, ws, ws_bytes, st);
+    int dev = 0, n_sm = 0;
+    SG_CUDA_TRY(cudaGetDevice(&dev));
+    SG_CUDA_TRY(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
+    int64_t grid = (n_docs + K64_WARPS - 1) / K64_WARPS;
+    const int64_t cap = (int64_t)n_sm * 8;
+    if (grid > cap) grid = cap;
+    tfidf64_known_kernel<<<(unsigned)grid, K64_WARPS * 32, 0, st>>>(offsets, n_docs, vocab_keys, vocab_size,
+                                                                    scratch_key, scratch_tf, scratch_col, row_nnz);
+    SG_LAUNCH_CHECK();
+    const int rc = transform_indptr(n_docs, row_nnz, indptr, ws, ws_bytes, st);
+    if (rc != SG_OK) return rc;
+    tfidf64_place_kernel<<<(unsigned)((n_docs + 7) / 8), 256, 0, st>>>(n_docs, offsets, indptr, scratch_col, indices);
     SG_LAUNCH_CHECK();
     return SG_OK;
 }
