@@ -468,6 +468,39 @@ int sg_rescore_refined_floor(int64_t n_cand, const int32_t *cand_row, const int3
                              const int32_t *row_len /*[dev] per left row id*/, float floor_margin,
                              float floor_margin_per_feature, unsigned long long *floor_dropped /*[dev] 1 or NULL*/,
                              void *stream);
+/* Arg-max re-score (match_nearest): per left row the right row of the largest exact score, without a top-n
+ * selection.  row_best[r - row_begin] [dev, zeroed by the caller before the first launch, kept across launches] holds
+ * the order-preserving bits of the largest score > keep_threshold (and >= row_floor[r] when row_floor is set) row r
+ * has met (atomicMax).  A pair is written to (keep_row, keep_col, score_out) only if its score is at least that
+ * running best, so every pair equal to the row's final best is written (the best only rises) and
+ * sg_nearest_master(nnz, keep_col, keep_row, score, n_rows, ...) over the written pairs gives the lowest column
+ * among them.  *keep_count [dev] += pairs written.  The floor arguments are those of sg_rescore_floor /
+ * sg_rescore_refined_floor (row_floor NULL: none); the refined form re-tests candidates as sg_rescore_refined.
+ * No mirror, no row counts. */
+int sg_rescore_nearest(int64_t n_cand, const int32_t *cand_row, const int32_t *cand_col,
+                       const int64_t *a_indptr, const int32_t *a_indices, const void *a_val,
+                       const int64_t *b_indptr, const int32_t *b_indices, const void *b_val, int dtype,
+                       double *score_out /*[dev] n_cand*/, double keep_threshold, int32_t *keep_row /*[dev] n_cand*/,
+                       int32_t *keep_col /*[dev] n_cand*/, unsigned long long *keep_count /*[dev] 1*/,
+                       unsigned long long *row_best /*[dev] per left row - row_begin*/, int64_t row_begin,
+                       const float *row_floor /*[dev] per left row id, or NULL*/,
+                       unsigned long long *floor_dropped /*[dev] 1 or NULL*/, void *stream);
+int sg_rescore_refined_nearest(int64_t n_cand, const int32_t *cand_row, const int32_t *cand_col,
+                               const float *cand_partial /*[dev] n_cand*/,
+                               const void *left_group_norms /*[dev] fp16[16] per left row id*/,
+                               const void *right_group_norms /*[dev] fp16[16] per right row id*/,
+                               const float *row_threshold /*[dev] per left row id*/,
+                               const int64_t *a_indptr, const int32_t *a_indices, const void *a_val,
+                               const int64_t *b_indptr, const int32_t *b_indices, const void *b_val, int dtype,
+                               double *score_out /*[dev] n_cand*/, double keep_threshold,
+                               int32_t *keep_row /*[dev] n_cand*/, int32_t *keep_col /*[dev] n_cand*/,
+                               unsigned long long *keep_count /*[dev] 1*/,
+                               unsigned long long *refined_count /*[dev] 1 or NULL*/,
+                               unsigned long long *row_best /*[dev] per left row - row_begin*/, int64_t row_begin,
+                               const float *row_floor /*[dev] per left row id, or NULL*/,
+                               const int32_t *row_len /*[dev] per left row id, with row_floor*/, float floor_margin,
+                               float floor_margin_per_feature, unsigned long long *floor_dropped /*[dev] 1 or NULL*/,
+                               void *stream);
 
 /*
  * Per-row selection: keep score > threshold (strict, sg.py:729/:740), at most

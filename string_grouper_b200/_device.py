@@ -14,8 +14,10 @@ _TORCH = None
 
 # hand-written kernels launched so far (CUB scans / sorts and memsets are not counted); bench.py "gpu_launches"
 LAUNCH_COUNTS = {"postings": 0, "candidates": 0, "rescore": 0, "select": 0, "symmetrize": 0, "tfidf": 0,
-                 "rowdot": 0, "order": 0, "tiles": 0, "groups": 0, "gather": 0, "prune": 0, "dedup": 0}
+                 "rowdot": 0, "order": 0, "tiles": 0, "groups": 0, "gather": 0, "prune": 0, "dedup": 0,
+                 "nearest": 0}
 # "tiles": the tile-centric K2 (csrc/sg_tiles.cu): build, pack_left, filter, candidates
+# "nearest": the arg-max of cossim_nearest over the re-scored pairs (sg_nearest_master); "groups" counts get_groups'
 
 TRANSFER_BYTES = {"d2h": 0, "h2d": 0}      # bytes moved by the bulk copies (bench.py e2e accounting)
 
@@ -535,8 +537,55 @@ def prune_left_floor(A, B, hrank, row_begin, row_end, threshold, margin, margin_
     return p_idx, p_val, p_len, p_thr, p_xp, p_xg
 
 
+def cossim_nearest(A, B, threshold, stats=None, prune=None, acc=None, kernel=None, floor=None, tile_w=None,
+                   warps=None):
+    """For every row i of A: the row j of B with the largest exact score A_i . B_j > threshold, the lowest j among
+    equal scores (match_nearest, DESIGN.md §4 "Nearest row").  Returns host arrays (best int64 [n], -1 where no
+    score passes; score float64 [n], 0 there).
+
+    Runs cossim_topn's path with top_n = 1 (pruning levels, row chunks, candidate-buffer retry, the top-n floor under
+    `floor` / SG_B200_TOPN_FLOOR, the floor init without a threshold), but over the full product (no triangle, no
+    dedup) and with the arg-max re-score (sg_rescore_nearest / sg_rescore_refined_nearest) instead of the top-n
+    selection: the selection keeps the larger column among equal scores, the arg-max the smaller one."""
+    t = require_cuda()
+    n = A.shape[0]
+    if n == 0 or B.shape[0] == 0 or A.nnz == 0 or B.nnz == 0:
+        if A.shape[1] != B.shape[1]:
+            raise ValueError("dimension mismatch: left has %d features, right has %d" % (A.shape[1], B.shape[1]))
+        if stats is not None:
+            stats.update(nearest=True, topn_floor=False, n_nearest_written=0)
+        return np.full(n, -1, dtype=np.int64), np.zeros(n, dtype=np.float64)
+    best, score = cossim_topn(A, B, 1, threshold, tile_w=tile_w, warps=warps, stats=stats, prune=prune, acc=acc,
+                              kernel=kernel, floor=floor, dedup=False, nearest=True)
+    return tuple(to_host(best.to(t.int64), score))
+
+
+def _select_nearest(cand_row, cand_col, score, n_cand, row_best, stats):
+    """(best, score) of cossim_nearest from the pairs the arg-max re-score wrote (row ids from 0): the lowest column
+    among the written pairs whose score equals the row's best (sg_nearest_master with rows and columns swapped)."""
+    t = torch()
+    L = _lib.load()
+    n_rows = row_best.numel()
+    dev = row_best.device
+    best = _empty(n_rows, t.int32, dev)
+    ws_bytes = int(L.sg_nearest_master_workspace_bytes(n_rows))
+    ws = _empty(ws_bytes, t.uint8, dev)
+    _lib.check(L.sg_nearest_master(n_cand, _ptr(cand_col), _ptr(cand_row), _ptr(score), n_rows, _ptr(best), _ptr(ws),
+                                   ws_bytes, _stream()))
+    LAUNCH_COUNTS["nearest"] += 3
+    # row_best holds sg_rescore_nearest's order-preserving bits: a set top bit marks a non-negative double
+    bits = t.where(row_best < 0, row_best ^ t.iinfo(t.int64).min, ~row_best)
+    best = best[:n_rows]
+    best_score = t.where(best >= 0, bits.view(t.float64), t.zeros((), dtype=t.float64, device=dev))
+    mark(stats, "select")
+    if stats is not None:
+        stats["nearest"] = True
+        stats["select"] = "nearest"
+    return best, best_score
+
+
 def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, warps=None, stats=None,
-                prune=None, acc=None, kernel=None, floor=None, dedup=None):
+                prune=None, acc=None, kernel=None, floor=None, dedup=None, nearest=False):
     """C[i,:] = top_n{ j : A_i . B_j > threshold } for rows [row_begin,row_end) of A.
 
     Device counterpart of the whole block loop of StringGrouper._build_matches
@@ -553,6 +602,9 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
     selection (SELECT_MODE "rows", top_n <= sg_topn_rows_cap() / 2), runs the product over the distinct rows U of A
     and gives every row its group's list (DESIGN.md §4 "Identical rows"); the result is bit-identical.  "auto" takes it
     from DEDUP_MIN_ROWS rows on when at least DEDUP_MIN_SHARE of them repeat another row; True wherever it applies.
+
+    `nearest` (cossim_nearest; top_n = 1, all rows, dedup=False): the arg-max re-score replaces the top-n selection
+    and the result is cossim_nearest's (best, score).
     """
     t = require_cuda()
     L = _lib.load()
@@ -565,6 +617,9 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
     row_begin = int(row_begin)
     n_rows = max(row_end - row_begin, 0)
     dev = A.device
+    if nearest and (int(top_n) != 1 or row_begin != 0 or row_end != n_left):
+        # the arg-max indexes its per-row state and sg_nearest_master's output by the row id itself
+        raise ValueError("nearest needs top_n = 1 and all rows of the left matrix (use cossim_nearest)")
     top_n = int(min(int(top_n), n_right))
     dt = _lib.SG_DTYPE_F32 if A.dtype == np.float32 else _lib.SG_DTYPE_F64
     shape = (n_left, n_right)
@@ -582,9 +637,10 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
             raise ValueError("the top-n floor needs top_n <= 32 and non-negative matrices")
         if (kernel or "row").lower() != "row":
             raise ValueError("the top-n floor runs on the row kernel only")
+    row_best = t.zeros(n_rows, dtype=t.int64, device=dev) if nearest else None     # sg_rescore_nearest's running best
     if floor is True or (floor == "auto" and floor_ok and float(threshold) < 0.5 and n_rows >= FLOOR_MIN_ROWS):
         out = _cossim_topn_floor(A, B, top_n, float(threshold), row_begin, row_end, tile_w, stats, prune, acc,
-                                 decide=floor == "auto")
+                                 decide=floor == "auto", row_best=row_best)
         if out is not None:
             return out
     if stats is not None:
@@ -594,7 +650,7 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
     if dedup not in (None, "auto", True, False):
         raise ValueError("dedup must be None, 'auto', True or False, got %r" % (dedup,))
     groups = None
-    if (dedup is not False and A is B and row_begin == 0 and row_end == n_left and SELECT_MODE == "rows"
+    if (dedup is not False and not nearest and A is B and row_begin == 0 and row_end == n_left and SELECT_MODE == "rows"
             and top_n <= int(L.sg_topn_rows_cap()) // 2 and (dedup is True or n_left >= DEDUP_MIN_ROWS)):
         groups = row_groups(A)
         if dedup is True or n_left - groups["m"] >= DEDUP_MIN_SHARE * n_left:
@@ -660,8 +716,8 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
         tiles_per_group = max(64, int(GROUP_BYTES // max(4 * B.nnz / T, 1)) // 64 * 64)
     # Self-match over all rows: the score is symmetric, so only the triangle of pairs (i, j) with j at or after i in
     # the common processing order is computed (diag_rank = each row's position in it) and the re-score mirrors every
-    # kept pair.  Row ranges (shards) and two matrices keep the full product.
-    triangle = A is B and row_begin == 0 and row_end == n_left
+    # kept pair.  Row ranges (shards), two matrices and the arg-max of `nearest` keep the full product.
+    triangle = not nearest and A is B and row_begin == 0 and row_end == n_left
     if triangle:
         perm_a, diag_rank = perm_b, right_order(B)[2]
     else:
@@ -856,7 +912,18 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
         keep_row = _empty(n_out, t.int32, dev)
         keep_col = _empty(n_out, t.int32, dev)
         counters.zero_()
-        if refine and cand_part is not None and l_xg is not None:
+        if nearest and refine and cand_part is not None and l_xg is not None:
+            _lib.check(L.sg_rescore_refined_nearest(
+                n_cand, _ptr(cand_row), _ptr(cand_col), _ptr(cand_part), _ptr(l_xg), _ptr(B._heavy_groups),
+                _ptr(l_thr), _ptr(A.d_indptr), _ptr(A.d_indices), _ptr(A.d_val), _ptr(B.d_indptr), _ptr(B.d_indices),
+                _ptr(B.d_val), dt, _ptr(score), float(threshold), _ptr(keep_row), _ptr(keep_col), c_count, c_walk,
+                _ptr(row_best), row_begin, None, None, 0.0, 0.0, None, _stream()))
+        elif nearest:
+            _lib.check(L.sg_rescore_nearest(n_cand, _ptr(cand_row), _ptr(cand_col), _ptr(A.d_indptr),
+                                            _ptr(A.d_indices), _ptr(A.d_val), _ptr(B.d_indptr), _ptr(B.d_indices),
+                                            _ptr(B.d_val), dt, _ptr(score), float(threshold), _ptr(keep_row),
+                                            _ptr(keep_col), c_count, _ptr(row_best), row_begin, None, None, _stream()))
+        elif refine and cand_part is not None and l_xg is not None:
             _lib.check(L.sg_rescore_refined(n_cand, _ptr(cand_row), _ptr(cand_col), _ptr(cand_part), _ptr(l_xg),
                                             _ptr(B._heavy_groups), _ptr(l_thr), _ptr(A.d_indptr), _ptr(A.d_indices),
                                             _ptr(A.d_val), _ptr(B.d_indptr), _ptr(B.d_indices), _ptr(B.d_val), dt,
@@ -898,6 +965,10 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
         if use_tiles:
             stats["stage_bytes"] = tiles["stage_bytes"]
 
+    if nearest:
+        if stats is not None:
+            stats["n_nearest_written"] = n_above
+        return _select_nearest(cand_row, cand_col, score, n_cand, row_best, stats)
     if groups is not None:
         return _select_groups(cand_row, cand_col, score, n_cand, groups, top_n, shape, stats)
     return _select_topn(cand_row, cand_col, score, n_cand, row_cnt, max_row_cnt, row_begin, n_rows, top_n, threshold,
@@ -986,7 +1057,7 @@ def topn_floor_init(A, B, top_n, threshold, row_begin=0, row_end=None):
     return floor
 
 
-def _cossim_topn_floor(A, B, top_n, threshold, row_begin, row_end, tile_w, stats, prune, acc, decide):
+def _cossim_topn_floor(A, B, top_n, threshold, row_begin, row_end, tile_w, stats, prune, acc, decide, row_best=None):
     """cossim_topn with the top-n floor (DESIGN.md §4): row kernel, full product (no triangle), 8 warps per CTA.
 
     floor[r] is a proven lower bound of the exact score of row r's top_n-th best pair, raised by the candidates
@@ -998,7 +1069,10 @@ def _cossim_topn_floor(A, B, top_n, threshold, row_begin, row_end, tile_w, stats
 
     threshold <= 0 (no threshold): the floors start from topn_floor_init, the left rows are pruned against them
     before the first launch, and the candidates kernel bounds rows of more than 32 kept features by the block-max test
-    as well (SG_FLOOR_LONG_ROWS); the accumulator is fp32."""
+    as well (SG_FLOOR_LONG_ROWS); the accumulator is fp32.
+
+    `row_best` (cossim_nearest, top_n = 1): the arg-max re-score with the floor replaces the top-n selection.  Every
+    pair scoring at least the floor is re-scored, so all pairs tied at a row's best are among them."""
     t = require_cuda()
     L = _lib.load()
     n_left, n_right = A.shape[0], B.shape[0]
@@ -1126,7 +1200,18 @@ def _cossim_topn_floor(A, B, top_n, threshold, row_begin, row_end, tile_w, stats
         keep_row = _empty(n_c, t.int32, dev)
         keep_col = _empty(n_c, t.int32, dev)
         counters.zero_()
-        if refine and part_buf is not None and l_xg is not None:
+        if row_best is not None and refine and part_buf is not None and l_xg is not None:
+            _lib.check(L.sg_rescore_refined_nearest(
+                n_c, _ptr(row_buf), _ptr(col_buf), _ptr(part_buf), _ptr(l_xg), _ptr(B._heavy_groups), _ptr(l_thr),
+                _ptr(A.d_indptr), _ptr(A.d_indices), _ptr(A.d_val), _ptr(B.d_indptr), _ptr(B.d_indices),
+                _ptr(B.d_val), dt, _ptr(score), threshold, _ptr(keep_row), _ptr(keep_col), c_count, c_refined,
+                _ptr(row_best), row_begin, _ptr(floor_buf), _ptr(l_len), margin, margin_pf, c_dropped, _stream()))
+        elif row_best is not None:
+            _lib.check(L.sg_rescore_nearest(
+                n_c, _ptr(row_buf), _ptr(col_buf), _ptr(A.d_indptr), _ptr(A.d_indices), _ptr(A.d_val),
+                _ptr(B.d_indptr), _ptr(B.d_indices), _ptr(B.d_val), dt, _ptr(score), threshold, _ptr(keep_row),
+                _ptr(keep_col), c_count, _ptr(row_best), row_begin, _ptr(floor_buf), c_dropped, _stream()))
+        elif refine and part_buf is not None and l_xg is not None:
             _lib.check(L.sg_rescore_refined_floor(
                 n_c, _ptr(row_buf), _ptr(col_buf), _ptr(part_buf), _ptr(l_xg), _ptr(B._heavy_groups), _ptr(l_thr),
                 _ptr(A.d_indptr), _ptr(A.d_indices), _ptr(A.d_val), _ptr(B.d_indptr), _ptr(B.d_indices),
@@ -1221,6 +1306,10 @@ def _cossim_topn_floor(A, B, top_n, threshold, row_begin, row_end, tile_w, stats
         stats["n_row_chunks"] = n_chunks
         stats["tile_w"], stats["warps"], stats["n_tiles"] = tile_w, warps, T
         stats["tiles_per_group"] = tiles_per_group
+    if row_best is not None:
+        if stats is not None:
+            stats["n_nearest_written"] = n_keep
+        return _select_nearest(cand_row, cand_col, score, n_keep, row_best, stats)
     return _select_topn(cand_row, cand_col, score, n_keep, row_cnt, max_row_cnt, row_begin, n_rows, top_n, threshold,
                         (n_left, n_right), stats)
 

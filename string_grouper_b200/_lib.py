@@ -94,6 +94,10 @@ SIGNATURES = {
                                 _p]),
     "sg_rescore_refined_floor": (_i32, [_i64, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i32, _p, _f64, _p, _p,
                                         _p, _p, _p, _i64, _p, _p, _f32, _f32, _p, _p]),
+    "sg_rescore_nearest": (_i32, [_i64, _p, _p, _p, _p, _p, _p, _p, _p, _i32, _p, _f64, _p, _p, _p, _p, _i64, _p, _p,
+                                  _p]),
+    "sg_rescore_refined_nearest": (_i32, [_i64, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i32, _p, _f64, _p,
+                                          _p, _p, _p, _p, _i64, _p, _p, _f32, _f32, _p, _p]),
     "sg_topn_rows_cap": (_i32, []),
     "sg_row_count_max": (_i32, [_i64, _p, _p, _p]),
     "sg_topn_select_rows_workspace_bytes": (_sz, [_i64, _i64]),

@@ -67,6 +67,13 @@ class StringGrouperCorpus:
         kwargs['max_n_matches'] = 1
         return self.fit(master, duplicates, master_id, duplicates_id, **kwargs).get_groups()
 
+    def match_nearest(self, master: pd.Series, duplicates: pd.Series, master_id: Optional[pd.Series] = None,
+                      duplicates_id: Optional[pd.Series] = None, **kwargs) -> Union[pd.DataFrame, pd.Series]:
+        """match_nearest on this corpus.  With the corpus Series as `master` (a register lookup: which corpus entry
+        is each incoming string?) the corpus matrix is the right operand, and its row order and postings carry over
+        from call to call."""
+        return self._grouper(master, duplicates, master_id, duplicates_id, **kwargs)._match_nearest()
+
     def group_similar_strings(self, strings_to_group: pd.Series, string_ids: Optional[pd.Series] = None,
                               **kwargs) -> Union[pd.DataFrame, pd.Series]:
         return self.fit(strings_to_group, master_id=string_ids, **kwargs).get_groups()

@@ -776,7 +776,31 @@ __device__ __forceinline__ bool floor_keep(bool keep, int32_t r, double sc, cons
     return keep && !drop;
 }
 
-template <typename T, int VEC>
+// Arg-max re-score (sg_rescore_nearest / sg_rescore_refined_nearest): best[r - row_begin] holds the order-preserving
+// bits of the largest exact score row r has met so far (atomicMax; zero = none yet).  A pair above the threshold (and
+// the floor) is written only if its score is at least that running best.  The best only rises, so every pair whose
+// score equals the row's final best is written; sg_nearest_master then takes the lowest column among them.
+struct RescoreNearest : RescoreFloor {
+    unsigned long long *best;
+};
+
+__device__ __forceinline__ unsigned long long score_order_bits(double x) {
+    const unsigned long long b = (unsigned long long)__double_as_longlong(x);
+    return (b >> 63) ? ~b : (b | 0x8000000000000000ull);      // order-preserving map of IEEE doubles to unsigned
+}
+
+__device__ __forceinline__ bool nearest_keep(bool keep, int32_t r, int64_t row_begin, double sc,
+                                             const RescoreFloor &) {
+    return keep;
+}
+__device__ __forceinline__ bool nearest_keep(bool keep, int32_t r, int64_t row_begin, double sc,
+                                             const RescoreNearest &rn) {
+    if (!keep) return false;
+    const unsigned long long b = score_order_bits(sc);
+    return atomicMax(rn.best + (r - row_begin), b) <= b;
+}
+
+template <typename T, int VEC, typename RF = RescoreFloor>
 __global__ void __launch_bounds__(256, 8) rescore_kernel(int64_t n, const int32_t *__restrict__ cr, const int32_t *__restrict__ cc,
                                const int64_t *__restrict__ a_indptr, const int32_t *__restrict__ a_idx,
                                const T *__restrict__ a_val, const int64_t *__restrict__ b_indptr,
@@ -784,7 +808,7 @@ __global__ void __launch_bounds__(256, 8) rescore_kernel(int64_t n, const int32_
                                double *__restrict__ out, double keep_thr, int32_t *__restrict__ keep_row,
                                int32_t *__restrict__ keep_col, unsigned long long *__restrict__ keep_count,
                                unsigned long long *__restrict__ mirror_count, int32_t *__restrict__ row_cnt,
-                               int64_t row_begin, RescoreFloor rf) {
+                               int64_t row_begin, RF rf) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     int32_t r = 0, c = 0;
     double sc = 0.0;
@@ -801,6 +825,7 @@ __global__ void __launch_bounds__(256, 8) rescore_kernel(int64_t n, const int32_
     }
     if (!keep_count) return;
     if (rf.floor) keep = floor_keep(keep, r, sc, rf);
+    keep = nearest_keep(keep, r, row_begin, sc, rf);
     keep_pairs(keep, keep && mirror_count && r != c, r, c, sc, threadIdx.x & 31, keep_row, keep_col, out, keep_count,
                mirror_count, row_cnt, row_begin);
 }
@@ -827,7 +852,7 @@ __device__ __forceinline__ float group_dot(const uint4 *__restrict__ x, const ui
     return d * (1.f + 1e-5f) + 1e-6f;
 }
 
-template <typename T, int VEC>
+template <typename T, int VEC, typename RF = RescoreFloor>
 __global__ void __launch_bounds__(256, 8)
 rescore_refined_kernel(int64_t n, const int32_t *__restrict__ cr, const int32_t *__restrict__ cc,
                        const float *__restrict__ partial, const uint4 *__restrict__ xg,
@@ -838,7 +863,7 @@ rescore_refined_kernel(int64_t n, const int32_t *__restrict__ cr, const int32_t 
                        double keep_thr, int32_t *__restrict__ keep_row, int32_t *__restrict__ keep_col,
                        unsigned long long *__restrict__ keep_count, unsigned long long *__restrict__ refined_count,
                        unsigned long long *__restrict__ mirror_count, int32_t *__restrict__ row_cnt,
-                       int64_t row_begin, RescoreFloor rf) {
+                       int64_t row_begin, RF rf) {
     __shared__ uint16_t live[REFINE_CHUNK];
     __shared__ int n_live;
     const int lane = threadIdx.x & 31;
@@ -884,6 +909,7 @@ rescore_refined_kernel(int64_t n, const int32_t *__restrict__ cr, const int32_t 
             keep = sc > keep_thr;
         }
         if (rf.floor) keep = floor_keep(keep, r, sc, rf);
+        keep = nearest_keep(keep, r, row_begin, sc, rf);
         keep_pairs(keep, keep && mirror_count && r != c, r, c, sc, lane, keep_row, keep_col, out, keep_count,
                    mirror_count, row_cnt, row_begin);
     }
@@ -1322,11 +1348,12 @@ int sg_cossim_candidates_floor(const int64_t *a_indptr, const int32_t *a_len, co
 
 }  // extern "C"
 
+template <typename RF>
 static int rescore(int64_t n_cand, const int32_t *cand_row, const int32_t *cand_col, const int64_t *a_indptr,
                    const int32_t *a_indices, const void *a_val, const int64_t *b_indptr, const int32_t *b_indices,
                    const void *b_val, int dtype, double *score_out, double keep_threshold, int32_t *keep_row,
                    int32_t *keep_col, unsigned long long *keep_count, unsigned long long *mirror_count,
-                   int32_t *row_cnt, int64_t row_begin, void *stream_, const RescoreFloor &rf) {
+                   int32_t *row_cnt, int64_t row_begin, void *stream_, const RF &rf) {
     cudaStream_t st = (cudaStream_t)stream_;
     if (n_cand <= 0) return SG_OK;
     if (keep_count && (!keep_row || !keep_col)) return fail(SG_ERR_INVALID, "keep_count needs keep_row and keep_col");
@@ -1335,9 +1362,10 @@ static int rescore(int64_t n_cand, const int32_t *cand_row, const int32_t *cand_
     const unsigned grid = (unsigned)((n_cand + 255) / 256);
     const bool vec = ((uintptr_t)b_indices & 15) == 0;      // merge_dot_vec reads aligned 16-byte index vectors
 #define SG_RESCORE(T, VEC)                                                                                        \
-    rescore_kernel<T, VEC><<<grid, 256, 0, st>>>(n_cand, cand_row, cand_col, a_indptr, a_indices, (const T *)a_val, \
-                                                 b_indptr, b_indices, (const T *)b_val, score_out, keep_threshold,  \
-                                                 keep_row, keep_col, keep_count, mirror_count, row_cnt, row_begin, rf)
+    rescore_kernel<T, VEC, RF><<<grid, 256, 0, st>>>(n_cand, cand_row, cand_col, a_indptr, a_indices,               \
+                                                     (const T *)a_val, b_indptr, b_indices, (const T *)b_val,       \
+                                                     score_out, keep_threshold, keep_row, keep_col, keep_count,     \
+                                                     mirror_count, row_cnt, row_begin, rf)
     if (rf.floor && !keep_count) return fail(SG_ERR_INVALID, "row_floor needs keep_count");
     if (dtype == SG_DTYPE_F64) {
         if (vec) SG_RESCORE(double, 1);
@@ -1353,6 +1381,7 @@ static int rescore(int64_t n_cand, const int32_t *cand_row, const int32_t *cand_
     return SG_OK;
 }
 
+template <typename RF>
 static int rescore_refined(int64_t n_cand, const int32_t *cand_row, const int32_t *cand_col, const float *cand_partial,
                            const void *left_group_norms, const void *right_group_norms, const float *row_threshold,
                            const int64_t *a_indptr, const int32_t *a_indices, const void *a_val,
@@ -1360,7 +1389,7 @@ static int rescore_refined(int64_t n_cand, const int32_t *cand_row, const int32_
                            double *score_out, double keep_threshold, int32_t *keep_row, int32_t *keep_col,
                            unsigned long long *keep_count, unsigned long long *refined_count,
                            unsigned long long *mirror_count, int32_t *row_cnt, int64_t row_begin, void *stream_,
-                           const RescoreFloor &rf) {
+                           const RF &rf) {
     cudaStream_t st = (cudaStream_t)stream_;
     if (n_cand <= 0) return SG_OK;
     if (!keep_count || !keep_row || !keep_col) return fail(SG_ERR_INVALID, "keep_count, keep_row and keep_col are required");
@@ -1371,7 +1400,7 @@ static int rescore_refined(int64_t n_cand, const int32_t *cand_row, const int32_
     const unsigned grid = (unsigned)((n_cand + REFINE_CHUNK - 1) / REFINE_CHUNK);
     const bool vec = ((uintptr_t)b_indices & 15) == 0;
 #define SG_RESCORE(T, VEC)                                                                                         \
-    rescore_refined_kernel<T, VEC><<<grid, 256, 0, st>>>(                                                           \
+    rescore_refined_kernel<T, VEC, RF><<<grid, 256, 0, st>>>(                                                       \
         n_cand, cand_row, cand_col, cand_partial, (const uint4 *)left_group_norms, (const uint4 *)right_group_norms, \
         row_threshold, a_indptr, a_indices, (const T *)a_val, b_indptr, b_indices, (const T *)b_val, score_out,      \
         keep_threshold, keep_row, keep_col, keep_count, refined_count, mirror_count, row_cnt, row_begin, rf)
@@ -1441,6 +1470,43 @@ int sg_rescore_refined_floor(int64_t n_cand, const int32_t *cand_row, const int3
                            keep_threshold, keep_row, keep_col, keep_count, refined_count, nullptr, row_cnt, row_begin,
                            stream_, RescoreFloor{row_floor, row_len, floor_margin, floor_margin_per_feature,
                                                  floor_dropped});
+}
+
+int sg_rescore_nearest(int64_t n_cand, const int32_t *cand_row, const int32_t *cand_col, const int64_t *a_indptr,
+                       const int32_t *a_indices, const void *a_val, const int64_t *b_indptr, const int32_t *b_indices,
+                       const void *b_val, int dtype, double *score_out, double keep_threshold, int32_t *keep_row,
+                       int32_t *keep_col, unsigned long long *keep_count, unsigned long long *row_best,
+                       int64_t row_begin, const float *row_floor, unsigned long long *floor_dropped, void *stream_) {
+    if (!keep_count || !row_best) return fail(SG_ERR_INVALID, "keep_count and row_best are required");
+    RescoreNearest rn{};
+    rn.floor = row_floor;
+    rn.dropped = floor_dropped;
+    rn.best = row_best;
+    return rescore(n_cand, cand_row, cand_col, a_indptr, a_indices, a_val, b_indptr, b_indices, b_val, dtype,
+                   score_out, keep_threshold, keep_row, keep_col, keep_count, nullptr, nullptr, row_begin, stream_, rn);
+}
+
+int sg_rescore_refined_nearest(int64_t n_cand, const int32_t *cand_row, const int32_t *cand_col,
+                               const float *cand_partial, const void *left_group_norms, const void *right_group_norms,
+                               const float *row_threshold, const int64_t *a_indptr, const int32_t *a_indices,
+                               const void *a_val, const int64_t *b_indptr, const int32_t *b_indices, const void *b_val,
+                               int dtype, double *score_out, double keep_threshold, int32_t *keep_row,
+                               int32_t *keep_col, unsigned long long *keep_count, unsigned long long *refined_count,
+                               unsigned long long *row_best, int64_t row_begin, const float *row_floor,
+                               const int32_t *row_len, float floor_margin, float floor_margin_per_feature,
+                               unsigned long long *floor_dropped, void *stream_) {
+    if (!row_best) return fail(SG_ERR_INVALID, "row_best is required");
+    RescoreNearest rn{};
+    rn.floor = row_floor;
+    rn.row_len = row_len;
+    rn.margin = floor_margin;
+    rn.margin_pf = floor_margin_per_feature;
+    rn.dropped = floor_dropped;
+    rn.best = row_best;
+    return rescore_refined(n_cand, cand_row, cand_col, cand_partial, left_group_norms, right_group_norms,
+                           row_threshold, a_indptr, a_indices, a_val, b_indptr, b_indices, b_val, dtype, score_out,
+                           keep_threshold, keep_row, keep_col, keep_count, refined_count, nullptr, nullptr, row_begin,
+                           stream_, rn);
 }
 
 int sg_rowwise_dot(int64_t n_rows, const int64_t *a_indptr, const int32_t *a_indices, const void *a_val,

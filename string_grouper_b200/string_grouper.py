@@ -114,6 +114,21 @@ def match_most_similar(master: pd.Series, duplicates: pd.Series, master_id: Opti
                          **kwargs).fit().get_groups()
 
 
+def match_nearest(master: pd.Series, duplicates: pd.Series, master_id: Optional[pd.Series] = None,
+                  duplicates_id: Optional[pd.Series] = None, **kwargs) -> Union[pd.DataFrame, pd.Series]:
+    """For each string in duplicates the most similar string in master, as the reference documents
+    match_most_similar (ref:100-108): the master with the largest similarity above min_similarity (min_similarity
+    <= 0: above 0), the lowest master position among equal similarities, the duplicate itself where no master
+    qualifies.  Same vectoriser fit and same result frame as match_most_similar; `max_n_matches` is ignored.
+
+    match_most_similar keeps the reference's code instead, which keeps one duplicate per master: a duplicate whose
+    best master already holds a better-scoring duplicate comes back unmatched or with a worse master.  match_nearest
+    equals `StringGrouper(master, duplicates, ..., max_n_matches=len(duplicates)).fit().get_groups()` without
+    materialising every pair above the threshold."""
+    return StringGrouper(master, duplicates=duplicates, master_id=master_id, duplicates_id=duplicates_id,
+                         **kwargs)._match_nearest()
+
+
 def match_strings(master: pd.Series, duplicates: Optional[pd.Series] = None, master_id: Optional[pd.Series] = None,
                   duplicates_id: Optional[pd.Series] = None, **kwargs) -> pd.DataFrame:
     """All pairs with cosine similarity above min_similarity (ref:130-153)."""
@@ -443,6 +458,12 @@ class StringGrouper(object):
         self.update_options(**kwargs)
         return self.fit().get_groups()
 
+    def match_nearest(self, master, duplicates, master_id=None, duplicates_id=None, **kwargs):
+        """The module-level match_nearest on new data with these options merged with `kwargs`."""
+        self.reset_data(master, duplicates, master_id, duplicates_id)
+        self.update_options(**kwargs)
+        return self._match_nearest()
+
     def group_similar_strings(self, strings_to_group, string_ids=None, **kwargs):
         self.reset_data(strings_to_group, master_id=string_ids)
         self.update_options(**kwargs)
@@ -502,8 +523,6 @@ class StringGrouper(object):
     def _get_nearest_matches(self, ignore_index=False, replace_na=False) -> Union[pd.DataFrame, pd.Series]:
         """For each duplicate: the master with the highest similarity, lowest index on ties; the duplicate
         itself when nothing matched (ref:783-849)."""
-        prefix = MOST_SIMILAR_PREFIX
-        master_label = f'{prefix}{self._master.name if self._master.name else DEFAULT_MASTER_NAME}'
         n_dup = len(self._duplicates)
         pairs = self._matches_list
         best = np.full(n_dup, -1, dtype=np.int64)
@@ -519,6 +538,23 @@ class StringGrouper(object):
             first = np.ones(len(order), dtype=bool)
             first[1:] = d[order][1:] != d[order][:-1]
             best[d[order][first]] = m[order][first]
+        return self._nearest_frame(best, ignore_index, replace_na)
+
+    def _match_nearest(self) -> Union[pd.DataFrame, pd.Series]:
+        """match_nearest on the current data and options: duplicates x masters^T on the device, one arg-max per
+        duplicate row (_device.cossim_nearest), shaped by the same code as match_most_similar's result."""
+        if self._duplicates is None:
+            raise TypeError('match_nearest needs a duplicates Series')
+        master_matrix, duplicate_matrix = self._get_tf_idf_matrices(shard=False)
+        B = _device.as_device_csr(master_matrix)
+        A = _device.as_device_csr(duplicate_matrix)
+        best, _ = _device.cossim_nearest(A, B, self._config.min_similarity, stats=self._last_stats)
+        return self._nearest_frame(best, self._config.ignore_index, self._config.replace_na)
+
+    def _nearest_frame(self, best, ignore_index, replace_na) -> Union[pd.DataFrame, pd.Series]:
+        """The result frame of _get_nearest_matches from best[d] = master position of duplicate d (-1: none)."""
+        prefix = MOST_SIMILAR_PREFIX
+        master_label = f'{prefix}{self._master.name if self._master.name else DEFAULT_MASTER_NAME}'
         hit = best >= 0
         pos = np.where(hit, best, 0)
         hit_s = pd.Series(hit)
@@ -530,7 +566,9 @@ class StringGrouper(object):
 
         def pick(master_series, dupe_series):
             # value of the matched master row, the duplicate's own value where nothing matched (ref:815-820)
-            if nullable(master_series):
+            if nullable(master_series) or _takes_as_str(master_series, dupe_series):
+                # Arrow `str` Series: the take keeps the dtype the object path below infers, without converting every
+                # master string to a Python object first (90 ms for 663k names, against about 1 ms for the take)
                 taken = pd.Series(master_series.array.take(pos))
                 return taken.where(hit_s, pd.Series(dupe_series.array))
             taken = pd.Series(master_series.to_numpy()[pos])
@@ -675,6 +713,15 @@ class StringGrouper(object):
 
 def _is_arrow_str(series):
     return isinstance(series.dtype, pd.StringDtype) and hasattr(series.array, "_pa_array")
+
+
+def _takes_as_str(master, duplicates):
+    """True when both Series are Arrow-backed with the dtype pandas infers for Python strings (pandas 3's default
+    `str`): then `pd.Series(master.to_numpy()[pos])` of _get_nearest_matches has that same dtype, and an Arrow take
+    gives the same column."""
+    inferred = pd.Series(np.array([''], dtype=object)).dtype
+    return (_is_arrow_str(master) and _is_arrow_str(duplicates)
+            and master.dtype == inferred and duplicates.dtype == inferred)
 
 
 def _gathered_array(series, offsets, data):
