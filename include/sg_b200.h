@@ -336,6 +336,30 @@ int sg_cossim_candidates_floor(const int64_t *a_indptr /*[dev]*/, const int32_t 
                                int warps_per_cta, float *row_floor /*[dev] per left row id*/, int top_n,
                                float floor_margin, float floor_margin_per_feature,
                                const int32_t *self_rank /*[dev] per row id, or NULL*/, int flags, void *stream);
+/*
+ * sg_cossim_candidates over a position range per left row (warps_per_cta = 8): row i reports only the columns at
+ * positions [lo_pos[i], hi_pos[i]) of the right processing order (`perm_b`), so a product restricted to pairs that
+ * share a block id sorts both sides by (block id, row order) and passes the row's block as its range; in a
+ * self-match lo_pos[i] is the row's own position (the triangle, as diag_rank).  Tiles wholly outside the range leave
+ * the block-max test, the columns outside it are not reported, and no work item is handed out for a column-tile group
+ * the range does not reach.  Work items are exact when lo_pos and hi_pos do not decrease along perm_a.
+ * `group_items` [dev] scratch of 2 * (sg_num_tiles()/tiles_per_group, rounded up) + 1 entries.
+ */
+int sg_cossim_candidates_range(const int64_t *a_indptr /*[dev]*/, const int32_t *a_len /*[dev] or NULL*/,
+                               const int32_t *a_indices /*[dev]*/, const float *a_val32 /*[dev]*/,
+                               int64_t row_begin, int64_t row_end, const int32_t *perm_a /*[dev] or NULL*/,
+                               int64_t n_right, int64_t n_cols, const void *bucket_dir /*[dev]*/,
+                               const void *bucket_maxw /*[dev]*/, const void *postings /*[dev]*/,
+                               const int32_t *perm_b /*[dev] or NULL*/, int tile_w, int acc_dtype, float a_scale,
+                               float cand_threshold, const float *cand_threshold_row /*[dev] per row id, or NULL*/,
+                               const float *pruned_norm_row /*[dev] per row id, or NULL*/,
+                               const float *tile_bound /*[dev]*/, int64_t tiles_per_group,
+                               const int32_t *lo_pos /*[dev] per left row id*/,
+                               const int32_t *hi_pos /*[dev] per left row id*/,
+                               unsigned long long *group_items /*[dev] scratch*/, int32_t *cand_row /*[dev] cap*/,
+                               int32_t *cand_col /*[dev] cap*/, float *cand_partial /*[dev] cap or NULL*/,
+                               int64_t cand_cap, unsigned long long *cand_count /*[dev] 1*/,
+                               unsigned long long *row_queue /*[dev] 1*/, int warps_per_cta, void *stream);
 
 /* ------------------------------------------------------------------------- *
  * K2, tile-centric form (csrc/sg_tiles.cu) — the default for L2-normalised non-negative matrices (K1 output).

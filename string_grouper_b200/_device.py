@@ -158,6 +158,7 @@ class DeviceCSR:
         self._heavy_norm = None     # per-row norm over the heavy features (sg_heavy_norms)
         self._heavy_groups = None   # the same per group of heavy ranks, fp16[16] (sg_rescore_refined)
         self._dedup = None          # groups of bit-identical rows and the matrix of their representatives (row_groups)
+        self._blocked = None        # blocked order and its postings under one block-id tensor (blocked_right_side)
         self.nonneg = True          # no negative stored value (K1 output; checked for uploaded matrices)
 
     @property
@@ -320,32 +321,70 @@ def right_tiles(B):
 def right_side(B, tile_w):
     """Row order (heavy norm, signature), feature-major bucketed postings, bucket directory with block maxima and
     per-tile pruning bounds of the right matrix, cached on B."""
-    t = require_cuda()
-    L = _lib.load()
     hrank, perm, rank = right_order(B)
     if tile_w not in B._postings2:
-        n_rows, n_cols = B.shape
-        T = int(L.sg_num_tiles(n_rows, tile_w))
-        nb = T * (n_cols + 1) + 1
-        if nb >= 2**31 - 1:
-            raise OverflowError("posting bucket table too large: %d features x %d tiles" % (n_cols, T))
-        Tp = int(L.sg_num_tiles_padded(n_rows, tile_w))
-        bucket_ptr = _empty(nb, t.int32, B.device)
-        bucket_dir = _empty(2 * nb, t.int32, B.device)
-        bucket_maxw = _empty((n_cols + 1) * Tp, t.float16, B.device)
-        post = _empty(max(B.nnz, 1), t.int32, B.device)
-        ws_bytes = int(L.sg_postings_workspace_bytes(B.nnz, n_cols, T))
-        ws = _empty(ws_bytes, t.uint8, B.device)
-        _lib.check(L.sg_postings_build(n_rows, n_cols, B.nnz, _ptr(B.d_indptr), _ptr(B.d_indices), _ptr(B.d_val32),
-                                       _ptr(rank), tile_w, B.base, 1.0 / max(B.norm_bound, 1.0), _ptr(bucket_ptr),
-                                       _ptr(bucket_dir), _ptr(bucket_maxw), _ptr(post),
-                                       _ptr(ws), ws_bytes, _stream()))
-        LAUNCH_COUNTS["postings"] += 4
-        bound = t.zeros(Tp, dtype=t.float32, device=B.device)
-        _lib.check(L.sg_tile_bounds(n_rows, _ptr(perm), _ptr(B._heavy_norm), tile_w, _ptr(bound), _stream()))
-        LAUNCH_COUNTS["prune"] += 1
-        B._postings2[tile_w] = (bucket_dir, bucket_maxw, post, T, bound)     # bucket_ptr is only needed for the build
+        B._postings2[tile_w] = _build_postings(B, perm, rank, tile_w)
     return (hrank, perm, rank) + B._postings2[tile_w]
+
+
+def blocked_right_side(B, block_ids, tile_w):
+    """right_side for the blocked order: B's rows stably sorted by block id (int32 device tensor, one per row), so
+    the usual order holds inside every block.  Cached on B under the block-id tensor itself, next to the unblocked
+    caches: (hrank, perm, rank, bucket_dir, bucket_maxw, post, T, tile_bound, sorted block ids)."""
+    t = require_cuda()
+    hrank, perm, _ = right_order(B)
+    c = B._blocked
+    if c is None or c["ids"] is not block_ids:
+        perm_k = blocked_order(perm, block_ids)
+        rank_k = t.empty_like(perm_k)
+        rank_k[perm_k.long()] = t.arange(perm_k.numel(), dtype=t.int32, device=B.device)
+        c = B._blocked = {"ids": block_ids, "perm": perm_k, "rank": rank_k,
+                          "sorted": block_ids[perm_k.long()].contiguous(), "postings": {}}
+    if tile_w not in c["postings"]:
+        c["postings"][tile_w] = _build_postings(B, c["perm"], c["rank"], tile_w)
+    return (hrank, c["perm"], c["rank"]) + c["postings"][tile_w] + (c["sorted"],)
+
+
+def blocked_order(perm, block_ids):
+    """The processing order `perm` (position -> row id) stably sorted by the rows' block ids: blocks in ascending id,
+    the order of `perm` inside each block."""
+    t = torch()
+    return perm[t.sort(block_ids[perm.long()], stable=True).indices].contiguous()
+
+
+def block_ranges(sorted_ids, block_ids):
+    """(lo, hi) int32 per row: the first and one-past-last positions of the row's block id among the right rows'
+    ids in their blocked order (`sorted_ids`, ascending); lo == hi where no right row has the id."""
+    t = torch()
+    return (t.searchsorted(sorted_ids, block_ids, out_int32=True),
+            t.searchsorted(sorted_ids, block_ids, right=True, out_int32=True))
+
+
+def _build_postings(B, perm, rank, tile_w):
+    """(bucket_dir, bucket_maxw, post, T, tile_bound) of B in the processing order (perm, rank)."""
+    t = require_cuda()
+    L = _lib.load()
+    n_rows, n_cols = B.shape
+    T = int(L.sg_num_tiles(n_rows, tile_w))
+    nb = T * (n_cols + 1) + 1
+    if nb >= 2**31 - 1:
+        raise OverflowError("posting bucket table too large: %d features x %d tiles" % (n_cols, T))
+    Tp = int(L.sg_num_tiles_padded(n_rows, tile_w))
+    bucket_ptr = _empty(nb, t.int32, B.device)
+    bucket_dir = _empty(2 * nb, t.int32, B.device)
+    bucket_maxw = _empty((n_cols + 1) * Tp, t.float16, B.device)
+    post = _empty(max(B.nnz, 1), t.int32, B.device)
+    ws_bytes = int(L.sg_postings_workspace_bytes(B.nnz, n_cols, T))
+    ws = _empty(ws_bytes, t.uint8, B.device)
+    _lib.check(L.sg_postings_build(n_rows, n_cols, B.nnz, _ptr(B.d_indptr), _ptr(B.d_indices), _ptr(B.d_val32),
+                                   _ptr(rank), tile_w, B.base, 1.0 / max(B.norm_bound, 1.0), _ptr(bucket_ptr),
+                                   _ptr(bucket_dir), _ptr(bucket_maxw), _ptr(post),
+                                   _ptr(ws), ws_bytes, _stream()))
+    LAUNCH_COUNTS["postings"] += 4
+    bound = t.zeros(Tp, dtype=t.float32, device=B.device)
+    _lib.check(L.sg_tile_bounds(n_rows, _ptr(perm), _ptr(B._heavy_norm), tile_w, _ptr(bound), _stream()))
+    LAUNCH_COUNTS["prune"] += 1
+    return bucket_dir, bucket_maxw, post, T, bound      # bucket_ptr is only needed for the build
 
 
 class DeviceMatches:
@@ -585,7 +624,7 @@ def _select_nearest(cand_row, cand_col, score, n_cand, row_best, stats):
 
 
 def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, warps=None, stats=None,
-                prune=None, acc=None, kernel=None, floor=None, dedup=None, nearest=False):
+                prune=None, acc=None, kernel=None, floor=None, dedup=None, nearest=False, block_ids=None):
     """C[i,:] = top_n{ j : A_i . B_j > threshold } for rows [row_begin,row_end) of A.
 
     Device counterpart of the whole block loop of StringGrouper._build_matches
@@ -605,6 +644,13 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
 
     `nearest` (cossim_nearest; top_n = 1, all rows, dedup=False): the arg-max re-score replaces the top-n selection
     and the result is cossim_nearest's (best, score).
+
+    `block_ids` (a pair of int32 device tensors, one id per row of A and one per row of B; the same tensor twice for a
+    self-match): only the pairs whose two rows have equal ids are eligible, and C[i,:] is the top_n of those (DESIGN.md
+    §4 "Blocks").  Both sides run in the blocked processing order (block id, then the usual order), every left row
+    reports the positions of its block among the right rows only (sg_cossim_candidates_range), and the scores are
+    those of the unblocked product bit for bit.  The top-n floor, the identical-rows dedup and the tile kernel are not
+    taken: floor=True, dedup=True and kernel="tiles" raise ValueError, SG_B200_KERNEL=tiles runs the row kernel.
     """
     t = require_cuda()
     L = _lib.load()
@@ -623,9 +669,29 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
     top_n = int(min(int(top_n), n_right))
     dt = _lib.SG_DTYPE_F32 if A.dtype == np.float32 else _lib.SG_DTYPE_F64
     shape = (n_left, n_right)
+    blocked = block_ids is not None
+    if blocked:
+        ids_a, ids_b = block_ids
+        if nearest:
+            raise ValueError("cossim_nearest takes no block ids")
+        for ids, n, side in ((ids_a, n_left, "left"), (ids_b, n_right, "right")):
+            if ids.dtype != t.int32 or ids.dim() != 1 or ids.numel() != n or ids.device != dev:
+                raise ValueError("block ids of the %s matrix must be %d int32 values on %s" % (side, n, dev))
+        if (A is B) != (ids_a is ids_b):
+            raise ValueError("a self-match takes one block-id tensor for both sides, two matrices take two")
+        if floor is True:
+            raise ValueError("the top-n floor does not run with block ids")
+        if dedup is True:
+            raise ValueError("the identical-rows dedup does not run with block ids")
+        if kernel is not None and kernel.lower() == "tiles":
+            raise ValueError("the tile kernel does not run with block ids")
+        kernel = "row"
+        floor = dedup = False
     if n_rows == 0 or n_right == 0 or top_n <= 0 or A.nnz == 0 or B.nnz == 0:
         z32 = _empty(1, t.int32, dev)
         return DeviceMatches(shape, z32, z32, _empty(1, t.float64, dev), 0, 0)
+    if stats is not None:
+        stats["blocks"] = blocked
 
     if floor not in (None, "auto", True, False):
         raise ValueError("floor must be None, 'auto', True or False, got %r" % (floor,))
@@ -708,17 +774,38 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
         mask_words = int(L.sg_tiles_mask_words(n_right))
     else:
         tile_w, warps = pick_tile(n_right, tile_w, warps, 2 if acc == "u16" else 4, n_left=n_rows)
+        if blocked:
+            warps = 8               # the range variant of the candidates kernel is built for 8 warps
         # the bucket directory holds one entry per (feature, tile): widen the tiles until it stays below MAX_BUCKETS
         while (-(-n_right // tile_w)) * (B.shape[1] + 1) > MAX_BUCKETS and tile_w < 32768:
             tile_w *= 2
-        hrank, perm_b, _, bucket_dir, bucket_maxw, post, T, tile_bound = right_side(B, tile_w)
+        if blocked:
+            hrank, perm_b, rank_b, bucket_dir, bucket_maxw, post, T, tile_bound, sorted_ids = \
+                blocked_right_side(B, ids_b, tile_w)
+        else:
+            hrank, perm_b, _, bucket_dir, bucket_maxw, post, T, tile_bound = right_side(B, tile_w)
         # column tiles per work group (a multiple of 64): the group's posting buckets should stay L2-resident
         tiles_per_group = max(64, int(GROUP_BYTES // max(4 * B.nnz / T, 1)) // 64 * 64)
     # Self-match over all rows: the score is symmetric, so only the triangle of pairs (i, j) with j at or after i in
     # the common processing order is computed (diag_rank = each row's position in it) and the re-score mirrors every
     # kept pair.  Row ranges (shards), two matrices and the arg-max of `nearest` keep the full product.
     triangle = not nearest and A is B and row_begin == 0 and row_end == n_left
-    if triangle:
+    hi_pos = None
+    if blocked:
+        # every left row reports the positions [lo, hi) of its block among the sorted right ids (in the triangle lo is
+        # the row's own position); the left rows run in the same blocked order, so lo and hi grow along perm_a
+        lo_pos, hi_pos = block_ranges(sorted_ids, ids_a)
+        if triangle:
+            perm_a, diag_rank = perm_b, rank_b          # the row's own position, inside its block
+        else:
+            perm_a = blocked_order(row_order(A, hrank, row_begin, row_end, want_rank=False)[0], ids_a)
+            diag_rank = lo_pos
+        # (left row, right row) pairs the launches visit, cumulated along perm_a: the density limit and row chunks
+        pair_cum = np.zeros(n_rows + 1, dtype=np.int64)
+        pair_cum[1:] = to_host(t.cumsum((hi_pos - diag_rank)[perm_a.long()].long(), 0))[0]
+        if stats is not None:
+            stats["n_blocks_used"] = int(t.unique(ids_a if triangle else t.cat([ids_a, ids_b])).numel())
+    elif triangle:
         perm_a, diag_rank = perm_b, right_order(B)[2]
     else:
         perm_a, _ = row_order(A, hrank, row_begin, row_end, want_rank=False)
@@ -731,7 +818,9 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
     dummy = _empty(1, t.int32, dev)
     pruned = {}
     group_items = None
-    if triangle and not use_tiles:
+    if blocked:
+        group_items = _empty(2 * -(-T // tiles_per_group) + 1, t.int64, dev)
+    elif triangle and not use_tiles:
         group_items = _empty(-(-T // tiles_per_group) + 1, t.int64, dev)
 
     def launch_tiles(perm, n, row_buf, col_buf, capacity):
@@ -759,6 +848,15 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
             return launch_tiles(perm, re_ - rb, row_buf, col_buf, capacity)
         l_idx, l_val, l_len, l_thr, l_xp, _ = pruned["arrays"]
         counters.zero_()
+        if blocked:
+            _lib.check(L.sg_cossim_candidates_range(
+                _ptr(A.d_indptr), _ptr(l_len), _ptr(l_idx), _ptr(l_val), rb, re_, _ptr(perm), n_right, A.shape[1],
+                _ptr(bucket_dir), _ptr(bucket_maxw), _ptr(post), _ptr(perm_b), tile_w, acc_code,
+                max(B.norm_bound, 1.0), thr_c, _ptr(l_thr), _ptr(l_xp), _ptr(tile_bound), tiles_per_group,
+                _ptr(diag_rank), _ptr(hi_pos), _ptr(group_items), _ptr(row_buf), _ptr(col_buf), _ptr(partial_buf),
+                capacity, c_count, c_queue, warps, _stream()))
+            LAUNCH_COUNTS["candidates"] += 1
+            return
         _lib.check(L.sg_cossim_candidates(
             _ptr(A.d_indptr), _ptr(l_len), _ptr(l_idx), _ptr(l_val), rb, re_, _ptr(perm), n_right,
             A.shape[1], _ptr(bucket_dir), _ptr(bucket_maxw), _ptr(post), _ptr(perm_b), tile_w, acc_code,
@@ -805,12 +903,16 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
     est = None
     first = None          # (cand_row, cand_col, n_cand) of a whole-range launch that needed no sizing pass
     search = True
-    # (row, column) pairs the launches visit: the triangle holds n (n + 1) / 2 of the n^2
-    dense = MAX_CAND_DENSITY * (n_rows * (n_rows + 1) / 2 if triangle else float(n_rows) * n_right)
+    # (row, column) pairs the launches visit: the triangle holds n (n + 1) / 2 of the n^2, blocks their own pairs
+    n_pairs = (float(pair_cum[-1]) if blocked else n_rows * (n_rows + 1) / 2 if triangle
+               else float(n_rows) * n_right)
+    dense = MAX_CAND_DENSITY * n_pairs
 
     def share(lo, hi):
         """fraction of the visited pairs that belong to the rows at positions [lo, hi) of the processing order (in the
         triangle the row at position r visits n - r columns)"""
+        if blocked:
+            return float(pair_cum[hi] - pair_cum[lo]) / max(n_pairs, 1.0)
         if not triangle:
             return (hi - lo) / n_rows
         return ((hi - lo) * n_rows - (lo + hi - 1) * (hi - lo) / 2) / (n_rows * (n_rows + 1) / 2)
@@ -825,7 +927,7 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
     # Candidates of the fixed-point row kernel carry their partial score: sg_rescore_refined re-tests each with the
     # grouped bound (csrc/sg_prune.cu) before its right row is read.
     refine = REFINE and not use_tiles and acc == "u16" and margin_pf > 0.0
-    if not fixed_cap and float(n_rows) * float(n_right) <= OPTIMISTIC_PAIRS:
+    if not fixed_cap and (n_pairs if blocked else float(n_rows) * float(n_right)) <= OPTIMISTIC_PAIRS:
         prune = levels[0]
         prepare(prune)
         cap0 = int(min(int(dense) + (1 << 22), chunk_cand))
@@ -973,6 +1075,15 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
         return _select_groups(cand_row, cand_col, score, n_cand, groups, top_n, shape, stats)
     return _select_topn(cand_row, cand_col, score, n_cand, row_cnt, max_row_cnt, row_begin, n_rows, top_n, threshold,
                         shape, stats)
+
+
+def block_id_tensors(ids, n_left, self_match):
+    """The block_ids pair of cossim_topn from the host ids of master ++ duplicates (int32): one tensor for both
+    sides of a self-match, the first n_left ids and the rest for two matrices."""
+    t = require_cuda()
+    TRANSFER_BYTES["h2d"] += ids.nbytes
+    d = t.from_numpy(np.ascontiguousarray(ids, dtype=np.int32)).to(t.device("cuda", t.cuda.current_device()))
+    return (d, d) if self_match else (d[:n_left], d[n_left:])
 
 
 FLOOR_INIT_WINDOW = 64      # right rows around each left row's position whose exact scores start its floor

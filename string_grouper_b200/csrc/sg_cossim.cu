@@ -257,6 +257,13 @@ __device__ __forceinline__ void apply_buckets(AccT *__restrict__ acc, const uint
 // `group_items` (with diag_rank): exclusive offsets of the work items per column-tile group (diag_items_kernel), so
 // that no item is handed out whose row has no tile at or above its rank in the group.
 //
+// Position range (cossim_candidates_range_kernel, `hi_pos` != NULL, with diag_rank as the lower end): row i reports
+// only the columns at positions in [diag_rank[i], hi_pos[i]) of the right processing order (a blocked product: both
+// sides sorted by block id first, the range is the row's block among the right rows).  Tiles wholly at or above hi
+// are left out of the block-max ballot, and in the tile holding hi the columns at or above it are not reported.
+// `group_items` then holds 2 * n_groups + 1 entries: the exclusive offsets of the work items per column-tile group and
+// the first ridx of each group (range_items_kernel); the items of group g are the rows first[g], first[g] + 1, ...
+//
 // Top-n floor (cossim_candidates_floor_kernel, top_n <= 32, non-negative weights): floor[row] is a proven lower bound
 // of the exact score of the row's top_n-th best pair; it only rises.  A pair whose exact score is below it cannot be
 // in the row's output, so the candidate threshold of the row becomes max(thr_row, floor - E_r - FLOOR_EPS), read again
@@ -303,7 +310,7 @@ __device__ __forceinline__ void floor_merge(float &kept, float x, int lane) {
     }
 }
 
-template <int NW, typename AccT, bool FLOOR, bool LONG_ROWS = false>
+template <int NW, typename AccT, bool FLOOR, bool LONG_ROWS = false, bool RANGE = false>
 __device__ __forceinline__ void
 candidates_body(const int64_t *__restrict__ a_indptr, const int32_t *__restrict__ a_len,
                 const int32_t *__restrict__ a_idx, const float *__restrict__ a_val, int64_t row_begin,
@@ -316,7 +323,7 @@ candidates_body(const int64_t *__restrict__ a_indptr, const int32_t *__restrict_
                 const unsigned long long *__restrict__ group_items, int32_t *__restrict__ cand_row,
                 int32_t *__restrict__ cand_col, float *__restrict__ cand_partial, unsigned long long cap,
                 unsigned long long *__restrict__ cand_count, unsigned long long *__restrict__ row_queue,
-                const FloorArgs &fa) {
+                const FloorArgs &fa, const int32_t *__restrict__ hi_pos = nullptr) {
     typedef AccOps<AccT> Ops;
     typedef typename Ops::val_t val_t;
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -351,6 +358,7 @@ candidates_body(const int64_t *__restrict__ a_indptr, const int32_t *__restrict_
         if (group_items) {
             while (item >= group_items[group + 1]) ++group;
             ridx = (int64_t)(item - group_items[group]);
+            if constexpr (RANGE) ridx += (int64_t)group_items[n_groups + 1 + group];
         } else {
             group = (int64_t)(item / (unsigned long long)n_rows);
             ridx = (int64_t)(item % (unsigned long long)n_rows);
@@ -379,9 +387,15 @@ candidates_body(const int64_t *__restrict__ a_indptr, const int32_t *__restrict_
         const float xp = xp_norm ? xp_norm[row] : 0.f;
         // tile ids, directory slots (T * V1 < 2^31, checked by sg_postings_build) and positions fit 32 bits
         const int t_begin = (int)(group * tiles_per_group);
-        const int t_end = (int)(t_begin + tiles_per_group < T ? t_begin + tiles_per_group : T);
+        int t_end = (int)(t_begin + tiles_per_group < T ? t_begin + tiles_per_group : T);
         // first column position this row reports (0: the full product); tile t holds positions [t*W, t*W + W)
         const int dr = diag_rank ? diag_rank[row] : 0;
+        int hr = 0;             // range: one past the last position the row reports; no tile from ceil(hr / W) on
+        if constexpr (RANGE) {
+            hr = hi_pos[row];
+            const int t_hi = (int)(((int64_t)hr + W - 1) / W);
+            if (t_hi < t_end) t_end = t_hi;
+        }
         const int t_first = (int)(((int64_t)dr / W) & ~63);            // first 64-tile batch at or above the rank
         const int tb_begin = t_first > t_begin ? t_first : t_begin;
 
@@ -509,6 +523,10 @@ candidates_body(const int64_t *__restrict__ a_indptr, const int32_t *__restrict_
                                 // the tile holding the rank: columns before it belong to earlier rows
                                 const int below = dr - (t * W + c * Ops::PER16);
                                 if (below > 0) m = below >= Ops::PER16 ? 0u : m & (~0u << below);
+                                if constexpr (RANGE) {      // the tile holding hi: columns from it on are not the row's
+                                    const int room = hr - (t * W + c * Ops::PER16);
+                                    if (room < Ops::PER16) m = room <= 0 ? 0u : m & ((1u << room) - 1u);
+                                }
                             }
                         }
                         if constexpr (FLOOR) {
@@ -590,6 +608,12 @@ __global__ void __launch_bounds__(NW * 32, min_ctas(NW))
     cossim_candidates_floor_long_kernel(SG_CAND_PARAMS, FloorArgs fa) {
     candidates_body<NW, AccT, true, true>(SG_CAND_ARGS, fa);
 }
+
+template <int NW, typename AccT>
+__global__ void __launch_bounds__(NW * 32, min_ctas(NW))
+    cossim_candidates_range_kernel(SG_CAND_PARAMS, const int32_t *__restrict__ hi_pos) {
+    candidates_body<NW, AccT, false, false, true>(SG_CAND_ARGS, FloorArgs{}, hi_pos);
+}
 #undef SG_CAND_PARAMS
 #undef SG_CAND_ARGS
 
@@ -630,6 +654,76 @@ __global__ void diag_items_kernel(int64_t n_groups, unsigned long long *__restri
             if (lane >= o) s += up;
         }
         if (g < n_groups) items[g] = run_sum + s - v;
+        run_sum += __shfl_sync(FULL, s, 31);
+    }
+    if (lane == 0) items[n_groups] = run_sum;
+}
+
+// Work items of a position-range product.  Row ridx has work in the groups from lo / group_cols to (hi - 1) / group_cols
+// (none when hi <= lo), so group g needs the items first[g] <= ridx < last[g], with last[g] = 1 + the largest ridx whose
+// first group is <= g and first[g] = the smallest ridx whose last group is >= g.  Every row with work in g lies in that
+// range whatever the order; the range holds no other row with work when lo and hi grow with ridx (the blocked
+// processing order and its slices and strides).
+// Pass 1: last[first group of ridx] = max(ridx + 1) in items[0, n_groups), (n_rows - first)[last group of ridx] =
+// max(n_rows - ridx) in items[n_groups + 1, 2 n_groups + 1), one atomic per warp and group.
+__global__ void range_groups_kernel(int64_t n_rows, const int32_t *__restrict__ perm_a, int64_t row_begin,
+                                    const int32_t *__restrict__ lo_pos, const int32_t *__restrict__ hi_pos,
+                                    int64_t group_cols, int64_t n_groups, unsigned long long *__restrict__ items) {
+    const int64_t ridx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    long long g0 = -1, g1 = -1;
+    if (ridx < n_rows) {
+        const int64_t row = perm_a ? perm_a[ridx] : row_begin + ridx;
+        const int64_t lo = lo_pos[row], hi = hi_pos[row];
+        if (hi > lo) {
+            g0 = lo / group_cols;
+            g1 = (hi - 1) / group_cols;
+        }
+    }
+    unsigned peers = __match_any_sync(FULL, g0);
+    if (g0 >= 0 && lane_id() == 31 - __clz(peers)) atomicMax(items + g0, (unsigned long long)(ridx + 1));
+    peers = __match_any_sync(FULL, g1);
+    if (g1 >= 0 && lane_id() == __ffs(peers) - 1)
+        atomicMax(items + n_groups + 1 + g1, (unsigned long long)(n_rows - ridx));
+}
+
+// Pass 2 (one warp): first[g] = n_rows - the suffix maximum of pass 1's second half, in place; then the prefix maximum
+// of last[], the items max(last[g] - first[g], 0) of each group and their exclusive sum in items[0, n_groups];
+// items[n_groups] = all items.
+__global__ void range_items_kernel(int64_t n_rows, int64_t n_groups, unsigned long long *__restrict__ items) {
+    const int lane = threadIdx.x;
+    unsigned long long *first = items + n_groups + 1;
+    unsigned long long run = 0;
+    for (int64_t g0 = 0; g0 < n_groups; g0 += 32) {           // from the last group down
+        const int64_t g = n_groups - 1 - g0 - lane;
+        unsigned long long v = g >= 0 ? first[g] : 0ull;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const unsigned long long up = __shfl_up_sync(FULL, v, o);
+            if (lane >= o && up > v) v = up;
+        }
+        if (run > v) v = run;
+        run = __shfl_sync(FULL, v, 31);
+        if (g >= 0) first[g] = (unsigned long long)n_rows - v;
+    }
+    unsigned long long run_max = 0, run_sum = 0;
+    for (int64_t g0 = 0; g0 < n_groups; g0 += 32) {
+        const int64_t g = g0 + lane;
+        unsigned long long v = g < n_groups ? items[g] : 0ull;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const unsigned long long up = __shfl_up_sync(FULL, v, o);
+            if (lane >= o && up > v) v = up;
+        }
+        if (run_max > v) v = run_max;
+        run_max = __shfl_sync(FULL, v, 31);
+        const unsigned long long c = (g < n_groups && v > first[g]) ? v - first[g] : 0ull;
+        unsigned long long s = c;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const unsigned long long up = __shfl_up_sync(FULL, s, o);
+            if (lane >= o) s += up;
+        }
+        if (g < n_groups) items[g] = run_sum + s - c;
         run_sum += __shfl_sync(FULL, s, 31);
     }
     if (lane == 0) items[n_groups] = run_sum;
@@ -1186,7 +1280,7 @@ int sg_postings_build(int64_t n_rows, int64_t n_cols, int64_t nnz, const int64_t
 
 }  // extern "C"
 
-template <int NW, typename AccT, bool FLOOR, bool LONG_ROWS = false>
+template <int NW, typename AccT, bool FLOOR, bool LONG_ROWS = false, bool RANGE = false>
 static int launch_candidates(const int64_t *a_indptr, const int32_t *a_len, const int32_t *a_indices,
                              const float *a_val32, int64_t row_begin, int64_t row_end, const int32_t *perm_a,
                              int64_t n_right, int64_t n_cols, const void *bucket_dir, const void *bucket_maxw,
@@ -1196,16 +1290,26 @@ static int launch_candidates(const int64_t *a_indptr, const int32_t *a_len, cons
                              const int32_t *diag_rank, unsigned long long *group_items,
                              int32_t *cand_row, int32_t *cand_col, float *cand_partial,
                              int64_t cand_cap, unsigned long long *cand_count, unsigned long long *row_queue,
-                             int n_sm, cudaStream_t st, const FloorArgs &fa) {
+                             int n_sm, cudaStream_t st, const FloorArgs &fa, const int32_t *hi_pos = nullptr) {
     const size_t smem = (size_t)NW * tile_w * sizeof(AccT);
     const void *kern;
-    if constexpr (LONG_ROWS) kern = (const void *)cossim_candidates_floor_long_kernel<NW, AccT>;
+    if constexpr (RANGE) kern = (const void *)cossim_candidates_range_kernel<NW, AccT>;
+    else if constexpr (LONG_ROWS) kern = (const void *)cossim_candidates_floor_long_kernel<NW, AccT>;
     else if constexpr (FLOOR) kern = (const void *)cossim_candidates_floor_kernel<NW, AccT>;
     else kern = (const void *)cossim_candidates_kernel<NW, AccT>;
     SG_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const int64_t T = sg_num_tiles(n_right, tile_w);
     const int64_t n_rows = row_end - row_begin;
-    if (diag_rank) {
+    if constexpr (RANGE) {
+        const int64_t n_groups = (T + tiles_per_group - 1) / tiles_per_group;
+        SG_CUDA_TRY(cudaMemsetAsync(group_items, 0, (size_t)(2 * n_groups + 1) * sizeof(unsigned long long), st));
+        range_groups_kernel<<<(unsigned)((n_rows + 255) / 256), 256, 0, st>>>(n_rows, perm_a, row_begin, diag_rank,
+                                                                              hi_pos, tiles_per_group * tile_w,
+                                                                              n_groups, group_items);
+        SG_LAUNCH_CHECK();
+        range_items_kernel<<<1, 32, 0, st>>>(n_rows, n_groups, group_items);
+        SG_LAUNCH_CHECK();
+    } else if (diag_rank) {
         const int64_t n_groups = (T + tiles_per_group - 1) / tiles_per_group;
         SG_CUDA_TRY(cudaMemsetAsync(group_items, 0, (size_t)(n_groups + 1) * sizeof(unsigned long long), st));
         diag_last_kernel<<<(unsigned)((n_rows + 255) / 256), 256, 0, st>>>(n_rows, perm_a, row_begin, diag_rank,
@@ -1226,7 +1330,9 @@ static int launch_candidates(const int64_t *a_indptr, const int32_t *a_len, cons
         tile_w, T, tiles_per_group, a_scale, thr_c, thr_row, xp_norm, tile_bound, diag_rank,                         \
         diag_rank ? group_items : nullptr, cand_row, cand_col, cand_partial, (unsigned long long)cand_cap, cand_count, \
         row_queue
-    if constexpr (LONG_ROWS)
+    if constexpr (RANGE)
+        cossim_candidates_range_kernel<NW, AccT><<<(unsigned)ctas, NW * 32, smem, st>>>(SG_KARGS, hi_pos);
+    else if constexpr (LONG_ROWS)
         cossim_candidates_floor_long_kernel<NW, AccT><<<(unsigned)ctas, NW * 32, smem, st>>>(SG_KARGS, fa);
     else if constexpr (FLOOR)
         cossim_candidates_floor_kernel<NW, AccT><<<(unsigned)ctas, NW * 32, smem, st>>>(SG_KARGS, fa);
@@ -1237,8 +1343,8 @@ static int launch_candidates(const int64_t *a_indptr, const int32_t *a_len, cons
     return SG_OK;
 }
 
-// fa == NULL: cossim_candidates_kernel; otherwise the floor variant (with `long_rows` the one that also bounds rows of
-// more than 32 kept features)
+// fa == NULL: cossim_candidates_kernel, or with `hi_pos` the position-range variant; otherwise the floor variant (with
+// `long_rows` the one that also bounds rows of more than 32 kept features)
 static int cossim_candidates(const int64_t *a_indptr, const int32_t *a_len, const int32_t *a_indices,
                              const float *a_val32, int64_t row_begin, int64_t row_end, const int32_t *perm_a,
                              int64_t n_right, int64_t n_cols, const void *bucket_dir, const void *bucket_maxw,
@@ -1248,7 +1354,8 @@ static int cossim_candidates(const int64_t *a_indptr, const int32_t *a_len, cons
                              int64_t tiles_per_group, const int32_t *diag_rank, unsigned long long *group_items,
                              int32_t *cand_row, int32_t *cand_col, float *cand_partial, int64_t cand_cap,
                              unsigned long long *cand_count, unsigned long long *row_queue, int warps_per_cta,
-                             void *stream_, const FloorArgs *fa, bool long_rows = false) {
+                             void *stream_, const FloorArgs *fa, bool long_rows = false,
+                             const int32_t *hi_pos = nullptr) {
     cudaStream_t st = (cudaStream_t)stream_;
     if (row_end <= row_begin || n_right <= 0) return SG_OK;
     if (acc_dtype != SG_ACC_F32 && acc_dtype != SG_ACC_U16)
@@ -1273,6 +1380,13 @@ static int cossim_candidates(const int64_t *a_indptr, const int32_t *a_len, cons
     a_indptr, a_len, a_indices, a_val32, row_begin, row_end, perm_a, n_right, n_cols, bucket_dir, bucket_maxw, \
         postings, perm_b, tile_w, tiles_per_group, a_scale, cand_threshold, cand_threshold_row, pruned_norm_row,      \
         tile_bound, diag_rank, group_items, cand_row, cand_col, cand_partial, cand_cap, cand_count, row_queue, n_sm, st
+    if (hi_pos) {
+        // the range variant is built for the default 8 warps only
+        if (warps_per_cta != 8) return fail(SG_ERR_INVALID, "the position-range variant runs with 8 warps per CTA");
+        if (!diag_rank || !group_items) return fail(SG_ERR_INVALID, "the position range needs lo_pos and group_items");
+        return acc_dtype == SG_ACC_U16 ? launch_candidates<8, uint16_t, false, false, true>(SG_ARGS, FloorArgs{}, hi_pos)
+                                       : launch_candidates<8, float, false, false, true>(SG_ARGS, FloorArgs{}, hi_pos);
+    }
     if (fa) {
         // the floor variant is built for the default 8 warps only
         if (warps_per_cta != 8) return fail(SG_ERR_INVALID, "the top-n floor variant runs with 8 warps per CTA");
@@ -1344,6 +1458,24 @@ int sg_cossim_candidates_floor(const int64_t *a_indptr, const int32_t *a_len, co
                              cand_threshold_row, pruned_norm_row, tile_bound, tiles_per_group, nullptr, nullptr,
                              cand_row, cand_col, cand_partial, cand_cap, cand_count, row_queue, warps_per_cta, stream_,
                              &fa, (flags & SG_FLOOR_LONG_ROWS) != 0);
+}
+
+int sg_cossim_candidates_range(const int64_t *a_indptr, const int32_t *a_len, const int32_t *a_indices,
+                               const float *a_val32, int64_t row_begin, int64_t row_end, const int32_t *perm_a,
+                               int64_t n_right, int64_t n_cols, const void *bucket_dir, const void *bucket_maxw,
+                               const void *postings, const int32_t *perm_b, int tile_w, int acc_dtype, float a_scale,
+                               float cand_threshold, const float *cand_threshold_row, const float *pruned_norm_row,
+                               const float *tile_bound, int64_t tiles_per_group, const int32_t *lo_pos,
+                               const int32_t *hi_pos, unsigned long long *group_items, int32_t *cand_row,
+                               int32_t *cand_col, float *cand_partial, int64_t cand_cap,
+                               unsigned long long *cand_count, unsigned long long *row_queue, int warps_per_cta,
+                               void *stream_) {
+    if (!lo_pos || !hi_pos || !group_items) return fail(SG_ERR_INVALID, "lo_pos, hi_pos and group_items are required");
+    return cossim_candidates(a_indptr, a_len, a_indices, a_val32, row_begin, row_end, perm_a, n_right, n_cols,
+                             bucket_dir, bucket_maxw, postings, perm_b, tile_w, acc_dtype, a_scale, cand_threshold,
+                             cand_threshold_row, pruned_norm_row, tile_bound, tiles_per_group, lo_pos, group_items,
+                             cand_row, cand_col, cand_partial, cand_cap, cand_count, row_queue, warps_per_cta, stream_,
+                             nullptr, false, hi_pos);
 }
 
 }  // extern "C"

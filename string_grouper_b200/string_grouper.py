@@ -100,18 +100,21 @@ def compute_pairwise_similarities(string_series_1: pd.Series, string_series_2: p
     return StringGrouper(string_series_1, string_series_2, **kwargs).dot()
 
 
-def group_similar_strings(strings_to_group: pd.Series, string_ids: Optional[pd.Series] = None,
-                          **kwargs) -> Union[pd.DataFrame, pd.Series]:
-    """Group representative for every string (ref:70-92)."""
-    return StringGrouper(strings_to_group, master_id=string_ids, **kwargs).fit().get_groups()
+def group_similar_strings(strings_to_group: pd.Series, string_ids: Optional[pd.Series] = None, *,
+                          keys: Optional[pd.Series] = None, **kwargs) -> Union[pd.DataFrame, pd.Series]:
+    """Group representative for every string (ref:70-92).  With `keys` (blocking keys, see StringGrouper) only
+    strings of equal keys are matched, so no group spans two keys."""
+    return StringGrouper(strings_to_group, master_id=string_ids, master_keys=keys, **kwargs).fit().get_groups()
 
 
 def match_most_similar(master: pd.Series, duplicates: pd.Series, master_id: Optional[pd.Series] = None,
-                       duplicates_id: Optional[pd.Series] = None, **kwargs) -> Union[pd.DataFrame, pd.Series]:
-    """Most similar master string for every duplicate; forces max_n_matches=1 like ref:120."""
+                       duplicates_id: Optional[pd.Series] = None, *, master_keys: Optional[pd.Series] = None,
+                       duplicates_keys: Optional[pd.Series] = None, **kwargs) -> Union[pd.DataFrame, pd.Series]:
+    """Most similar master string for every duplicate; forces max_n_matches=1 like ref:120.  With blocking keys
+    (see StringGrouper) a duplicate is matched only against masters of its own key."""
     kwargs['max_n_matches'] = 1
     return StringGrouper(master, duplicates=duplicates, master_id=master_id, duplicates_id=duplicates_id,
-                         **kwargs).fit().get_groups()
+                         master_keys=master_keys, duplicates_keys=duplicates_keys, **kwargs).fit().get_groups()
 
 
 def match_nearest(master: pd.Series, duplicates: pd.Series, master_id: Optional[pd.Series] = None,
@@ -130,15 +133,24 @@ def match_nearest(master: pd.Series, duplicates: pd.Series, master_id: Optional[
 
 
 def match_strings(master: pd.Series, duplicates: Optional[pd.Series] = None, master_id: Optional[pd.Series] = None,
-                  duplicates_id: Optional[pd.Series] = None, **kwargs) -> pd.DataFrame:
-    """All pairs with cosine similarity above min_similarity (ref:130-153)."""
+                  duplicates_id: Optional[pd.Series] = None, *, master_keys: Optional[pd.Series] = None,
+                  duplicates_keys: Optional[pd.Series] = None, **kwargs) -> pd.DataFrame:
+    """All pairs with cosine similarity above min_similarity (ref:130-153); with blocking keys (see StringGrouper)
+    only the pairs of equal keys."""
     return StringGrouper(master, duplicates=duplicates, master_id=master_id, duplicates_id=duplicates_id,
-                         **kwargs).fit().get_matches()
+                         master_keys=master_keys, duplicates_keys=duplicates_keys, **kwargs).fit().get_matches()
 
 
 class StringGrouper(object):
+    """Blocking keys (`master_keys`, and `duplicates_keys` with `duplicates`: Series of hashable values, one per
+    string, aligned by position like `master_id`, whatever their index): a pair of strings is matched only when both
+    keys are present and equal; a missing key (None, NaN, pd.NA) matches no other string.  The vectoriser is fitted on
+    all strings as without keys, so every reported similarity equals the unkeyed one; `max_n_matches` counts the
+    matches of equal keys only.  A string's keys go with its data: reset_data and the match methods replace them."""
+
     def __init__(self, master: pd.Series, duplicates: Optional[pd.Series] = None,
-                 master_id: Optional[pd.Series] = None, duplicates_id: Optional[pd.Series] = None, **kwargs):
+                 master_id: Optional[pd.Series] = None, duplicates_id: Optional[pd.Series] = None, *,
+                 master_keys: Optional[pd.Series] = None, duplicates_keys: Optional[pd.Series] = None, **kwargs):
         self.is_build = False
         self._master = pd.Series(dtype=object)
         self._duplicates = None
@@ -155,18 +167,21 @@ class StringGrouper(object):
         self._matches_device = None      # match list in HBM as long as it equals _matches_list
         self._raw_device = None          # the callers' strings in HBM (packed UTF-8) when ingest left them untouched
         self._last_stats = {}
-        self._set_data(master, duplicates, master_id, duplicates_id)
+        self._block_ids = None           # int32 block id per string of master ++ duplicates (blocking keys), or None
+        self._set_data(master, duplicates, master_id, duplicates_id, master_keys, duplicates_keys)
         self._set_options(**kwargs)
         # ref:267 fits a vectoriser here and again in fit() (SURVEY §0 fact 9); the second fit gives the
         # identical vocabulary, so the device vectoriser runs once, inside fit().
 
     # ------------------------------------------------------------------ data / options (ref:269-363)
-    def _set_data(self, master, duplicates=None, master_id=None, duplicates_id=None):
+    def _set_data(self, master, duplicates=None, master_id=None, duplicates_id=None, master_keys=None,
+                  duplicates_keys=None):
         self.master = master
         self.duplicates = duplicates
         if not StringGrouper._is_input_data_combination_valid(duplicates, master_id, duplicates_id):
             raise Exception('List of data Series options is invalid')
         StringGrouper._validate_id_data(master, duplicates, master_id, duplicates_id)
+        self._block_ids = block_ids_of(master, duplicates, master_keys, duplicates_keys)
         self._master_id = master_id
         self._duplicates_id = duplicates_id
         self._left_Series = self._master
@@ -182,9 +197,10 @@ class StringGrouper(object):
         StringGrouper._validate_n_blocks(self._config.n_blocks)
         self.is_build = False
 
-    def reset_data(self, master, duplicates=None, master_id=None, duplicates_id=None):
-        """Replace the input Series, keeping the options (ref:310-323)."""
-        self._set_data(master, duplicates, master_id, duplicates_id)
+    def reset_data(self, master, duplicates=None, master_id=None, duplicates_id=None, *, master_keys=None,
+                   duplicates_keys=None):
+        """Replace the input Series and blocking keys, keeping the options (ref:310-323)."""
+        self._set_data(master, duplicates, master_id, duplicates_id, master_keys, duplicates_keys)
 
     def clear_data(self):
         self._master = None
@@ -237,7 +253,8 @@ class StringGrouper(object):
     # ------------------------------------------------------------------ the hot path
     def fit(self):
         """Vectorise, match, post-process; fills `_matches_list` (ref:380-431)."""
-        master_matrix, duplicate_matrix = self._get_tf_idf_matrices()
+        # a keyed product runs whole on every rank (its blocked row order spans all rows)
+        master_matrix, duplicate_matrix = self._get_tf_idf_matrices(shard=self._block_ids is None)
 
         guess = (max(1, round(len(self._left_Series) / 1e6)), max(1, round(len(self._right_Series) / 4e3)))
         if self._n_blocks is None:
@@ -342,7 +359,12 @@ class StringGrouper(object):
         A = _device.as_device_csr(master_matrix)
         B = A if duplicate_matrix is master_matrix else _device.as_device_csr(duplicate_matrix)
         rank, world_size = _dist.world()
-        if world_size > 1 and getattr(A, "row_offset", None) is not None:
+        if self._block_ids is not None:
+            # blocking keys: only pairs of equal block ids (the vectoriser and the scores are the unkeyed ones)
+            block_ids = _device.block_id_tensors(self._block_ids, A.shape[0], B is A)
+            out = _device.cossim_topn(A, B, self._max_n_matches, self._config.min_similarity,
+                                      stats=self._last_stats, block_ids=block_ids)
+        elif world_size > 1 and getattr(A, "row_offset", None) is not None:
             # K1 was sharded: A already IS this rank's block of left rows.  The rank-local product runs guarded: a
             # rank that fails (OverflowError ...) tells the others before anybody enters the gather.
             out = _dist.guarded(_device.cossim_topn, A, B, self._max_n_matches, self._config.min_similarity,
@@ -448,13 +470,17 @@ class StringGrouper(object):
         return self._get_nearest_matches(ignore_index=ignore_index, replace_na=replace_na)
 
     # corpus-reusing variants (ref:546-644); like the reference they refit on the new data
-    def match_strings(self, master, duplicates=None, master_id=None, duplicates_id=None, **kwargs) -> pd.DataFrame:
-        self.reset_data(master, duplicates, master_id, duplicates_id)
+    def match_strings(self, master, duplicates=None, master_id=None, duplicates_id=None, *, master_keys=None,
+                      duplicates_keys=None, **kwargs) -> pd.DataFrame:
+        self.reset_data(master, duplicates, master_id, duplicates_id, master_keys=master_keys,
+                        duplicates_keys=duplicates_keys)
         self.update_options(**kwargs)
         return self.fit().get_matches()
 
-    def match_most_similar(self, master, duplicates, master_id=None, duplicates_id=None, **kwargs):
-        self.reset_data(master, duplicates, master_id, duplicates_id)
+    def match_most_similar(self, master, duplicates, master_id=None, duplicates_id=None, *, master_keys=None,
+                           duplicates_keys=None, **kwargs):
+        self.reset_data(master, duplicates, master_id, duplicates_id, master_keys=master_keys,
+                        duplicates_keys=duplicates_keys)
         self.update_options(**kwargs)
         return self.fit().get_groups()
 
@@ -464,8 +490,8 @@ class StringGrouper(object):
         self.update_options(**kwargs)
         return self._match_nearest()
 
-    def group_similar_strings(self, strings_to_group, string_ids=None, **kwargs):
-        self.reset_data(strings_to_group, master_id=string_ids)
+    def group_similar_strings(self, strings_to_group, string_ids=None, *, keys=None, **kwargs):
+        self.reset_data(strings_to_group, master_id=string_ids, master_keys=keys)
         self.update_options(**kwargs)
         return self.fit().get_groups()
 
@@ -709,6 +735,33 @@ class StringGrouper(object):
             raise Exception('Both master and master_id must be pandas.Series of the same length.')
         if duplicates is not None and duplicates_id is not None and len(duplicates) != len(duplicates_id):
             raise Exception('Both duplicates and duplicates_id must be pandas.Series of the same length.')
+
+
+def block_ids_of(master, duplicates=None, master_keys=None, duplicates_keys=None):
+    """int32 block id of every string of master ++ duplicates from the blocking keys (None without keys).
+
+    The keys of both sides are factorised together (pd.factorize), by position: equal values get equal ids on either
+    side, and every missing value (None, NaN, pd.NA) an id of its own, so it matches no other string."""
+    if duplicates_keys is not None and duplicates is None:
+        raise ValueError('duplicates_keys needs duplicates')
+    if duplicates is not None and (master_keys is None) != (duplicates_keys is None):
+        raise ValueError('with duplicates, give both master_keys and duplicates_keys or neither')
+    if master_keys is None:
+        return None
+    sides = [(master, master_keys, 'master')] + ([] if duplicates is None else [(duplicates, duplicates_keys,
+                                                                                  'duplicates')])
+    for strings, keys, name in sides:
+        if not isinstance(keys, pd.Series):
+            raise TypeError(f'{name}_keys must be a pandas.Series')
+        if len(keys) != len(strings):
+            raise ValueError(f'{name}_keys has {len(keys)} values for {len(strings)} strings')
+    keys = pd.concat([k for _, k, _ in sides], ignore_index=True)
+    codes, uniques = pd.factorize(keys, use_na_sentinel=True)
+    missing = codes < 0
+    codes[missing] = len(uniques) + np.arange(int(missing.sum()))
+    if len(uniques) + int(missing.sum()) >= 2**31:
+        raise OverflowError('more than 2^31 - 1 distinct blocking keys')
+    return codes.astype(np.int32)
 
 
 def _is_arrow_str(series):
