@@ -688,6 +688,25 @@ int sg_rowwise_dot(int64_t n_rows, const int64_t *a_indptr, const int32_t *a_ind
                    const int64_t *b_indptr, const int32_t *b_indices, const void *b_val, int dtype,
                    double *out /*[dev] n_rows*/, void *stream);
 
+/* ------------------------------------------------------------------------- *
+ * Records: several string fields in one product (csrc/sg_fields.cu).  No reference counterpart: the reference
+ * compares one Series.  Every field is vectorised by K1 on its own; sg_fields_stack lays the fields' rows side by
+ * side into one CSR of n_rows rows:
+ *   out_indptr = exclusive scan of the summed row lengths (out_indptr[0] = 0);
+ *   row r holds field 0's entries of row r, then field 1's ..., field k's column ids + col_offset[k] and values
+ *   val * scale[k] in the matrix dtype (one rounding, no FMA; for SG_DTYPE_F32 scale[k] is first rounded to float);
+ *   out_val32 (or NULL for SG_DTYPE_F32, whose out_val is the fp32 array itself) = (float) of every value.
+ * indptr[k] / indices[k] / val[k] are HOST arrays of n_fields device pointers; indptr[k] has n_rows+1 absolute
+ * positions into indices[k] / val[k] (a row-range view need not start at 0).  scale[k] in (0, 1] and col_offset[k]
+ * are host arrays too.  Output arrays hold sum of the fields' row lengths entries.  1 <= n_fields <= SG_FIELDS_MAX.
+ * ------------------------------------------------------------------------- */
+#define SG_FIELDS_MAX 32
+size_t sg_fields_stack_workspace_bytes(int64_t n_rows);
+int sg_fields_stack(int n_fields, int64_t n_rows, const int64_t *const *indptr, const int32_t *const *indices,
+                    const void *const *val, const double *scale, const int32_t *col_offset, int dtype,
+                    int64_t *out_indptr /*[dev] n_rows+1*/, int32_t *out_indices /*[dev]*/, void *out_val /*[dev]*/,
+                    float *out_val32 /*[dev] or NULL*/, void *ws, size_t ws_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -15,9 +15,10 @@ _TORCH = None
 # hand-written kernels launched so far (CUB scans / sorts and memsets are not counted); bench.py "gpu_launches"
 LAUNCH_COUNTS = {"postings": 0, "candidates": 0, "rescore": 0, "select": 0, "symmetrize": 0, "tfidf": 0,
                  "rowdot": 0, "order": 0, "tiles": 0, "groups": 0, "gather": 0, "prune": 0, "dedup": 0,
-                 "nearest": 0}
+                 "nearest": 0, "fields": 0}
 # "tiles": the tile-centric K2 (csrc/sg_tiles.cu): build, pack_left, filter, candidates
 # "nearest": the arg-max of cossim_nearest over the re-scored pairs (sg_nearest_master); "groups" counts get_groups'
+# "fields": the weighted stacking of a records call (sg_fields_stack)
 
 TRANSFER_BYTES = {"d2h": 0, "h2d": 0}      # bytes moved by the bulk copies (bench.py e2e accounting)
 
@@ -1621,6 +1622,67 @@ def rowwise_dot(A, B):
                                 _ptr(B.d_indices), _ptr(B.d_val), dt, _ptr(out), _stream()))
     LAUNCH_COUNTS["rowdot"] += 1
     return out[:A.shape[0]].cpu().numpy().astype(A.dtype, copy=False)
+
+
+def field_scales(weights, dtype):
+    """scale_k = sqrt(w_k / sum w) in float64, rounded to the matrix dtype for float32 matrices: the factor
+    sg_fields_stack multiplies field k's values by."""
+    w = np.asarray(weights, dtype=np.float64)
+    s = np.sqrt(w / w.sum())
+    return s.astype(np.float32).astype(np.float64) if np.dtype(dtype) == np.float32 else s
+
+
+def stack_fields(parts, scales):
+    """Fields laid side by side (csrc/sg_fields.cu): `parts` are DeviceCSR of the same rows, one per field, in field
+    order; field k's columns start after the vocabularies of the fields before it and its values are multiplied by
+    scales[k] (field_scales).  Returns the stacked DeviceCSR (norm_bound 1: DESIGN.md §4 "Fields")."""
+    t = require_cuda()
+    L = _lib.load()
+    k = len(parts)
+    if not 1 <= k <= _lib.SG_FIELDS_MAX:
+        raise ValueError("%d fields; one call stacks 1 to %d" % (k, _lib.SG_FIELDS_MAX))
+    n_rows = parts[0].shape[0]
+    np_dtype = parts[0].dtype
+    if any(p.shape[0] != n_rows or p.dtype != np_dtype for p in parts):
+        raise ValueError("the fields must have the same rows and dtype")
+    col_off = np.concatenate([[0], np.cumsum([p.shape[1] for p in parts])]).astype(np.int64)
+    if col_off[-1] >= 2**31:
+        raise OverflowError("the fields' vocabularies hold %d columns together; int32 indices overflow" % col_off[-1])
+    nnz = sum(p.nnz for p in parts)
+    if nnz >= 2**31 - 1:
+        raise OverflowError("the stacked matrix has %d stored values; int32 indices overflow" % nnz)
+    dev = parts[0].device
+    indptr = _empty(n_rows + 1, t.int64, dev)
+    indices = _empty(nnz, t.int32, dev)
+    val32 = _empty(nnz, t.float32, dev)
+    f64 = np_dtype == np.float64
+    val = _empty(nnz, t.float64, dev) if f64 else val32
+    ws_bytes = int(L.sg_fields_stack_workspace_bytes(n_rows))
+    ws = _empty(ws_bytes, t.uint8, dev)
+    ptrs = ctypes.c_void_p * k
+    _lib.check(L.sg_fields_stack(
+        k, n_rows, ptrs(*[p.d_indptr.data_ptr() for p in parts]), ptrs(*[p.d_indices.data_ptr() for p in parts]),
+        ptrs(*[p.d_val.data_ptr() for p in parts]), (ctypes.c_double * k)(*[float(s) for s in scales]),
+        (ctypes.c_int32 * k)(*[int(c) for c in col_off[:-1]]), _lib.SG_DTYPE_F64 if f64 else _lib.SG_DTYPE_F32,
+        _ptr(indptr), _ptr(indices), _ptr(val), _ptr(val32) if f64 else None, _ptr(ws), ws_bytes, _stream()))
+    LAUNCH_COUNTS["fields"] += 2
+    return DeviceCSR((n_rows, int(col_off[-1])), indptr, indices, val, val32, nnz, np_dtype, 1.0)
+
+
+def pair_scores(A, B, M):
+    """float64 numpy [M.nnz]: the exact score of every pair (d_row[i], d_col[i]) of the device match list M between
+    the rows of A and B — sg_rescore without a threshold (keep_count NULL), in the order scipy's A @ B.T adds."""
+    t = require_cuda()
+    L = _lib.load()
+    if not M.nnz:
+        return np.zeros(0, np.float64)
+    out = _empty(M.nnz, t.float64, M.d_row.device)
+    dt = _lib.SG_DTYPE_F32 if A.dtype == np.float32 else _lib.SG_DTYPE_F64
+    _lib.check(L.sg_rescore(M.nnz, _ptr(M.d_row), _ptr(M.d_col), _ptr(A.d_indptr), _ptr(A.d_indices), _ptr(A.d_val),
+                            _ptr(B.d_indptr), _ptr(B.d_indices), _ptr(B.d_val), dt, _ptr(out), 0.0, None, None, None,
+                            None, None, 0, _stream()))
+    LAUNCH_COUNTS["rescore"] += 1
+    return to_host(out[:M.nnz])[0]
 
 
 def sklearn_idf(df, n_docs_fit, dtype):

@@ -14,6 +14,7 @@ library then uses its own process group, checks that every rank was given the sa
 exchanges an error flag before every collective so that a rank that failed locally takes the others down with a
 clear exception instead of leaving them waiting.
 """
+import contextlib
 import os
 import zlib
 
@@ -46,6 +47,17 @@ def group():
         _STATE["group"] = dist.new_group(ranks=list(range(dist.get_world_size())))
         _STATE["group_for"] = default
     return _STATE["group"]
+
+
+@contextlib.contextmanager
+def local():
+    """Inside the block world() is (0, 1): the work runs whole in this process, whatever the other ranks do."""
+    saved = _STATE["enabled"]
+    _STATE["enabled"] = False
+    try:
+        yield
+    finally:
+        _STATE["enabled"] = saved
 
 
 def world():

@@ -27,6 +27,7 @@ SG_FLOOR_SEED = 1
 SG_FLOOR_LONG_ROWS = 2
 SG_SYMBOL_UNKNOWN = 0xffffffff      # a query symbol outside the fitted alphabet (K1 transform)
 SG_LUT_UNKNOWN = 0xfe
+SG_FIELDS_MAX = 32                  # fields one sg_fields_stack call lays side by side
 
 _i64 = ctypes.c_int64
 _i32 = ctypes.c_int
@@ -127,6 +128,8 @@ SIGNATURES = {
     "sg_gather_offsets": (_i32, [_p, _i64, _i64, _p, _p, _p, _sz, _p]),
     "sg_gather_bytes": (_i32, [_p, _p, _i64, _i64, _p, _p, _p, _p]),
     "sg_rowwise_dot": (_i32, [_i64, _p, _p, _p, _p, _p, _p, _i32, _p, _p]),
+    "sg_fields_stack_workspace_bytes": (_sz, [_i64]),
+    "sg_fields_stack": (_i32, [_i32, _i64, _p, _p, _p, _p, _p, _i32, _p, _p, _p, _p, _p, _sz, _p]),
 }
 
 _LIB = None

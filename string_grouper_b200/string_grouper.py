@@ -641,21 +641,7 @@ class StringGrouper(object):
                 rep_values = _gathered_array(self._master, *rhost)
         else:
             # the list was edited by add_match / remove_match: host statement of the same rule
-            pairs = self._matches_list
-            rows, cols = pairs.master_side.to_numpy(), pairs.dupe_side.to_numpy()
-            graph = csr_matrix((np.full(len(pairs), 1), (rows, cols)), shape=(n, n))
-            _, group = connected_components(csgraph=graph, directed=True)
-            if centroid:
-                graph.data = pairs['similarity'].to_numpy()
-                weight = np.asarray(graph.sum(axis=1)).squeeze(axis=1)
-                order = np.lexsort((np.arange(n), -weight, group))   # per group: weight desc, first index on ties
-            else:
-                order = np.lexsort((np.arange(n), group))            # per group: first index
-            head = np.ones(n, dtype=bool)
-            head[1:] = group[order][1:] != group[order][:-1]
-            rep_of_group = np.empty(group.max() + 1 if n else 0, dtype=np.int64)
-            rep_of_group[group[order][head]] = order[head]
-            rep = rep_of_group[group]
+            rep = self._host_group_reps(n, centroid)
 
         prefix = GROUP_REP_PREFIX
         label = f'{prefix}{self._master.name}' if self._master.name else prefix[:-1]
@@ -679,6 +665,25 @@ class StringGrouper(object):
             output = pd.concat([self._master_id.iloc[rep].rename(id_label).reset_index(drop=True), output], axis=1)
         output.index = self._master.index
         return output
+
+    def _host_group_reps(self, n, centroid):
+        """Representative position of every string's group from the host match list: connected components, then per
+        group the largest similarity sum (centroid) or the first index, the first index on ties."""
+        pairs = self._matches_list
+        rows, cols = pairs.master_side.to_numpy(), pairs.dupe_side.to_numpy()
+        graph = csr_matrix((np.full(len(pairs), 1), (rows, cols)), shape=(n, n))
+        _, group = connected_components(csgraph=graph, directed=True)
+        if centroid:
+            graph.data = pairs['similarity'].to_numpy()
+            weight = np.asarray(graph.sum(axis=1)).squeeze(axis=1)
+            order = np.lexsort((np.arange(n), -weight, group))   # per group: weight desc, first index on ties
+        else:
+            order = np.lexsort((np.arange(n), group))            # per group: first index
+        head = np.ones(n, dtype=bool)
+        head[1:] = group[order][1:] != group[order][:-1]
+        rep_of_group = np.empty(group.max() + 1 if n else 0, dtype=np.int64)
+        rep_of_group[group[order][head]] = order[head]
+        return rep_of_group[group]
 
     def _get_indices_of(self, master_side: str, dupe_side: str) -> Tuple[pd.Series, pd.Series]:
         master_strings = self._master
