@@ -189,26 +189,27 @@ int64_t sg_num_tiles_padded(int64_t n_right, int tile_w);
 /*
  * Right matrix -> tile-major postings (the transpose that sp_matmul_topn performs on
  * `Bi.T`, sg.py:727/:738, done once and laid out for the kernel).  The right rows are taken in the
- * order `rank` (position of every row in heavy-feature signature order, sg_row_order; NULL = input
- * order): column tile t holds positions [t*tile_w, (t+1)*tile_w); bucket (f, t) = the docs of feature f
- * inside tile t (in no particular order), at bucket_ptr[f*T + t] (feature-major, T = sg_num_tiles); a posting is 4 bytes:
- * position - t*tile_w in the low 16 bits, the weight rounded to fp16 in the high 16 bits (candidate
- * scores only need to be within the caller's margin; every candidate is re-scored exactly).  `bucket_dir` (optional) receives the same directory as aligned
- * 8-byte entries {int32 start, u16 length, fp16 largest |weight| of the bucket}, T*(n_cols+1) of them, the form
- * sg_cossim_candidates reads.  `bucket_maxw` receives the largest weights again as fp16 rows, one row of
- * sg_num_tiles_padded() entries per feature (zero padded), which sg_cossim_candidates streams to skip every
- * (left row, column tile) pair whose score bound sum_f |a_f| * max|w_(f,t)| cannot reach the candidate
- * threshold.  tile_w <= 32768.
+ * order `perm` (row at every position of the heavy-feature signature order, sg_row_order; NULL = input
+ * order): column tile t holds positions [t*tile_w, (t+1)*tile_w), T = sg_num_tiles.  The postings of tile t lie
+ * contiguously, sorted by feature; bucket (f, t) = the docs of feature f inside tile t (in no particular order).
+ * A posting is 4 bytes: position - t*tile_w in the low 16 bits, the weight rounded to fp16 in the high 16 bits
+ * (candidate scores only need to be within the caller's margin; every candidate is re-scored exactly).
+ * `bucket_dir` receives the directory as aligned 8-byte entries {int32 start, u16 length, fp16 largest |weight| of
+ * the bucket} at f*T + t (feature-major), T*(n_cols+1) of them, the form sg_cossim_candidates reads; empty buckets
+ * are all zero.  `bucket_maxw` receives the largest weights again as fp16 rows, one row of sg_num_tiles_padded()
+ * entries per feature (zero padded), which sg_cossim_candidates streams to skip every (left row, column tile) pair
+ * whose score bound sum_f |a_f| * max|w_(f,t)| cannot reach the candidate threshold.  tile_w <= 32768.
+ * A tile is sorted in shared memory by one CTA; a tile of more postings than fit there (long rows, wide tiles) is
+ * sorted in global memory instead, and `n_spilled` (optional, zeroed by the caller) counts those tiles.
  * `indptr` may be a row-range view (indptr_base = indptr[0]).
  */
 size_t sg_postings_workspace_bytes(int64_t nnz, int64_t n_cols, int64_t n_tiles);
 int sg_postings_build(int64_t n_rows, int64_t n_cols, int64_t nnz, const int64_t *indptr /*[dev]*/,
                       const int32_t *indices /*[dev]*/, const float *val32 /*[dev]*/,
-                      const int32_t *rank /*[dev] or NULL*/, int tile_w, int64_t indptr_base,
+                      const int32_t *perm /*[dev] or NULL*/, int tile_w, int64_t indptr_base,
                       float w_scale /* weights are multiplied by this before the fp16 rounding: 1 / max|w| */,
-                      int32_t *bucket_ptr /*[dev] T*(n_cols+1)+1*/,
-                      void *bucket_dir /*[dev] T*(n_cols+1)*8 B or NULL*/,
-                      void *bucket_maxw /*[dev] (n_cols+1)*Tp*2 B or NULL*/, void *postings /*[dev] nnz*4 B*/,
+                      void *bucket_dir /*[dev] T*(n_cols+1)*8 B*/, void *bucket_maxw /*[dev] (n_cols+1)*Tp*2 B*/,
+                      void *postings /*[dev] nnz*4 B*/, int32_t *n_spilled /*[dev] or NULL*/,
                       void *ws /*[dev]*/, size_t ws_bytes, void *stream);
 
 /*

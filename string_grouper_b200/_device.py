@@ -324,7 +324,7 @@ def right_side(B, tile_w):
     per-tile pruning bounds of the right matrix, cached on B."""
     hrank, perm, rank = right_order(B)
     if tile_w not in B._postings2:
-        B._postings2[tile_w] = _build_postings(B, perm, rank, tile_w)
+        B._postings2[tile_w] = _build_postings(B, perm, tile_w)
     return (hrank, perm, rank) + B._postings2[tile_w]
 
 
@@ -342,7 +342,7 @@ def blocked_right_side(B, block_ids, tile_w):
         c = B._blocked = {"ids": block_ids, "perm": perm_k, "rank": rank_k,
                           "sorted": block_ids[perm_k.long()].contiguous(), "postings": {}}
     if tile_w not in c["postings"]:
-        c["postings"][tile_w] = _build_postings(B, c["perm"], c["rank"], tile_w)
+        c["postings"][tile_w] = _build_postings(B, c["perm"], tile_w)
     return (hrank, c["perm"], c["rank"]) + c["postings"][tile_w] + (c["sorted"],)
 
 
@@ -361,31 +361,32 @@ def block_ranges(sorted_ids, block_ids):
             t.searchsorted(sorted_ids, block_ids, right=True, out_int32=True))
 
 
-def _build_postings(B, perm, rank, tile_w):
-    """(bucket_dir, bucket_maxw, post, T, tile_bound) of B in the processing order (perm, rank)."""
+def _build_postings(B, perm, tile_w, n_spilled=None):
+    """(bucket_dir, bucket_maxw, post, T, tile_bound) of B in the processing order `perm` (position -> row).  `n_spilled`
+    (optional int32 device tensor of one zeroed element) counts the tiles too large to be sorted in shared memory."""
     t = require_cuda()
     L = _lib.load()
     n_rows, n_cols = B.shape
     T = int(L.sg_num_tiles(n_rows, tile_w))
-    nb = T * (n_cols + 1) + 1
+    nb = T * (n_cols + 1)
     if nb >= 2**31 - 1:
         raise OverflowError("posting bucket table too large: %d features x %d tiles" % (n_cols, T))
     Tp = int(L.sg_num_tiles_padded(n_rows, tile_w))
-    bucket_ptr = _empty(nb, t.int32, B.device)
     bucket_dir = _empty(2 * nb, t.int32, B.device)
     bucket_maxw = _empty((n_cols + 1) * Tp, t.float16, B.device)
     post = _empty(max(B.nnz, 1), t.int32, B.device)
     ws_bytes = int(L.sg_postings_workspace_bytes(B.nnz, n_cols, T))
     ws = _empty(ws_bytes, t.uint8, B.device)
     _lib.check(L.sg_postings_build(n_rows, n_cols, B.nnz, _ptr(B.d_indptr), _ptr(B.d_indices), _ptr(B.d_val32),
-                                   _ptr(rank), tile_w, B.base, 1.0 / max(B.norm_bound, 1.0), _ptr(bucket_ptr),
-                                   _ptr(bucket_dir), _ptr(bucket_maxw), _ptr(post),
+                                   _ptr(perm), tile_w, B.base, 1.0 / max(B.norm_bound, 1.0),
+                                   _ptr(bucket_dir), _ptr(bucket_maxw), _ptr(post), _ptr(n_spilled),
                                    _ptr(ws), ws_bytes, _stream()))
-    LAUNCH_COUNTS["postings"] += 4
+    # tile counts, their scan, the per-tile sort, the segmented sort of the spilled tiles and their directory
+    LAUNCH_COUNTS["postings"] += 5
     bound = t.zeros(Tp, dtype=t.float32, device=B.device)
     _lib.check(L.sg_tile_bounds(n_rows, _ptr(perm), _ptr(B._heavy_norm), tile_w, _ptr(bound), _stream()))
     LAUNCH_COUNTS["prune"] += 1
-    return bucket_dir, bucket_maxw, post, T, bound      # bucket_ptr is only needed for the build
+    return bucket_dir, bucket_maxw, post, T, bound
 
 
 class DeviceMatches:

@@ -20,65 +20,177 @@
 namespace sg {
 
 // ---------------------------------------------------------------------------
-// postings build: feature-major buckets (feature, column tile) over the processing order of the right rows
+// postings build: one column tile at a time
 // ---------------------------------------------------------------------------
-// bucket = f * T + t (feature-major: the buckets a left row walks for one of its features over consecutive column
-// tiles are neighbours in the directory and in the posting array), t = rank[doc] / tile_w.
-// Pass 1: bucket sizes and the largest |weight| of every bucket.
-__global__ void postings_count_kernel(int64_t n_rows, const int64_t *__restrict__ indptr,
-                                      const int32_t *__restrict__ indices, const float *__restrict__ val,
-                                      const int32_t *__restrict__ rank, int W, int64_t T, float w_scale,
-                                      int32_t *__restrict__ cnt, uint32_t *__restrict__ maxw) {
-    const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-    if (row >= n_rows) return;
-    const int64_t t = (rank ? rank[row] : row) / W;
-    const int64_t p1 = indptr[row + 1];
-    for (int64_t p = indptr[row] + lane_id(); p < p1; p += 32) {
-        const int64_t b = (int64_t)indices[p] * T + t;
-        atomicAdd(cnt + b, 1);
-        // largest |weight| of the bucket as the fp16 value the kernel will see (non-negative halves order like integers)
-        atomicMax(maxw + b, (uint32_t)__half_as_ushort(__float2half_rn(fabsf(val[p] * w_scale))));
-    }
-}
-
-// Pass 2 (after the scan of the sizes): every posting takes the next free slot of its bucket, counting `cnt` down.
+// Column tile t holds the right rows perm[t*W .. t*W + W) of the processing order.  Its postings lie contiguously at
+// tile_off[t], sorted by feature; bucket (f, t) is the run of feature f among them.  Only the directory is
+// feature-major, dir[f * T + t]: the entries a left row reads for one of its features over consecutive column tiles
+// are neighbours.  Nothing is built per (feature, tile) pair beyond that: the caller clears the directory and the
+// block maxima, and every tile writes the entries of the features it holds.
+//
 // A posting is 4 bytes: the column inside the tile (16 bits) and the weight rounded to fp16 (16 bits).  The
 // candidate scores only have to be within CAND_MARGIN of the exact ones (every candidate is re-scored in the
 // matrix dtype): an fp16 weight is off by at most 2^-11 relative, so a score by at most 4.9e-4.  The order inside a
-// bucket is whatever the atomics make it (a bucket holds every column once; the fixed-point tiles add integers, so
-// the candidate set does not depend on it) — this replaced a 44-bit radix sort of all postings (1.1 of 2.6 ms).
-__global__ void postings_scatter_kernel(int64_t n_rows, const int64_t *__restrict__ indptr,
-                                        const int32_t *__restrict__ indices, const float *__restrict__ val,
-                                        const int32_t *__restrict__ rank, int W, int64_t T, float w_scale,
-                                        const int32_t *__restrict__ ptr, int32_t *__restrict__ cnt,
-                                        uint32_t *__restrict__ post) {
-    const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-    if (row >= n_rows) return;
-    const int64_t pos = rank ? rank[row] : row;
-    const int64_t t = pos / W;
-    const uint32_t local = (uint32_t)(pos - t * W);
-    const int64_t p1 = indptr[row + 1];
-    for (int64_t p = indptr[row] + lane_id(); p < p1; p += 32) {
-        const int64_t b = (int64_t)indices[p] * T + t;
-        const int slot = ptr[b] + atomicSub(cnt + b, 1) - 1;
-        post[slot] = ((uint32_t)__half_as_ushort(__float2half_rn(val[p] * w_scale)) << 16) | local;
+// bucket is arbitrary (a bucket holds every column once; the fixed-point tiles add integers, so the candidate set
+// does not depend on it).
+constexpr int PB_THREADS = 1024;
+constexpr int PB_ITEMS = 8;
+constexpr int PB_CAP = PB_THREADS * PB_ITEMS;   // postings of a tile sorted in shared memory; larger tiles: global
+constexpr size_t PB_SMEM = (size_t)PB_CAP * 8;  // keys + postings (the block sort's scratch reuses them)
+
+__device__ __forceinline__ uint32_t make_posting(float v, float w_scale, uint32_t local) {
+    return ((uint32_t)__half_as_ushort(__float2half_rn(v * w_scale)) << 16) | local;
+}
+
+// postings per tile, one warp per tile; tile_cnt[T] = 0 closes the exclusive scan into tile_off
+__global__ void postings_tile_count_kernel(int64_t n_rows, int64_t T, int W, const int64_t *__restrict__ indptr,
+                                           const int32_t *__restrict__ perm, int32_t *__restrict__ tile_cnt) {
+    const int64_t t = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (t > T) return;
+    int s = 0;      // < nnz < 2^31
+    if (t < T) {
+        const int64_t p1 = (t + 1) * W < n_rows ? (t + 1) * W : n_rows;
+        for (int64_t p = t * W + lane_id(); p < p1; p += 32) {
+            const int64_t row = perm ? perm[p] : p;
+            s += (int)(indptr[row + 1] - indptr[row]);
+        }
     }
+#pragma unroll
+    for (int o = 16; o; o >>= 1) s += __shfl_xor_sync(FULL, s, o);
+    if (lane_id() == 0) tile_cnt[t] = s;
+}
+
+// The directory entries of the runs of sorted keys[0, n) (postings pst[0, n), the first at posting index `start`):
+// one aligned 8-byte entry per (feature, tile) so that a lane fetches it in one load,
+// {int32 start, u16 length | fp16 largest |weight| << 16}, and the same maxima as fp16 rows of Tp tiles per feature
+// (what the block-max test streams).  |round(w)| = round(|w|), and non-negative halves order like integers.
+__device__ __forceinline__ void postings_emit_runs(const uint32_t *keys, const uint32_t *pst, int n, int start,
+                                                   int64_t t, int64_t T, int64_t Tp, int2 *__restrict__ dir,
+                                                   unsigned short *__restrict__ maxw_rows) {
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        const uint32_t f = keys[i];
+        if (i > 0 && keys[i - 1] == f) continue;
+        uint32_t m = 0;
+        int j = i;
+        for (; j < n && keys[j] == f; ++j) m = max(m, (pst[j] >> 16) & 0x7fffu);
+        dir[(int64_t)f * T + t] = make_int2(start + i, (int)(((uint32_t)(j - i) & 0xffffu) | (m << 16)));
+        maxw_rows[(int64_t)f * Tp + t] = (unsigned short)m;
+    }
+}
+
+// Block radix sort by feature of the n <= PB_THREADS * ITEMS (key, posting) pairs in skey / spost, in place; the
+// sort's scratch reuses the same shared memory.  Items are taken in striped order and sorted as if blocked: a fixed
+// permutation of the input, so the result is still deterministic.  Padding keys (all key_bits set, above every
+// feature) sort behind the n postings.
+template <int ITEMS>
+__device__ __forceinline__ void postings_sort_tile(uint32_t *skey, uint32_t *spost, int n, int key_bits) {
+    typedef cub::BlockRadixSort<uint32_t, PB_THREADS, ITEMS, uint32_t> Sort;
+    static_assert(sizeof(typename Sort::TempStorage) <= PB_SMEM, "block sort scratch exceeds the tile buffers");
+    const uint32_t pad = (uint32_t)((1ull << key_bits) - 1);
+    uint32_t keys[ITEMS], vals[ITEMS];
+#pragma unroll
+    for (int k = 0; k < ITEMS; ++k) {
+        const int i = k * PB_THREADS + threadIdx.x;
+        keys[k] = i < n ? skey[i] : pad;
+        vals[k] = i < n ? spost[i] : 0u;
+    }
+    __syncthreads();
+    Sort(*reinterpret_cast<typename Sort::TempStorage *>(skey)).SortBlockedToStriped(keys, vals, 0, key_bits);
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < ITEMS; ++k) {
+        const int i = k * PB_THREADS + threadIdx.x;
+        skey[i] = keys[k];
+        spost[i] = vals[k];
+    }
+}
+
+// One CTA per tile: the tile's (feature, posting) pairs in row order, then
+//   * up to PB_CAP of them: sorted by feature in shared memory, postings and directory entries written;
+//   * more: copied to big_key / big_post at tile_off[t] and big_end[t] = tile_off[t + 1], for the segmented sort
+//     (postings_big_dir_kernel finishes them); every other tile sets big_end[t] = tile_off[t], an empty segment.
+__global__ void __launch_bounds__(PB_THREADS)
+postings_tile_build_kernel(int64_t n_rows, int64_t T, int64_t Tp, int W, int key_bits,
+                           const int64_t *__restrict__ indptr, const int32_t *__restrict__ indices,
+                           const float *__restrict__ val, const int32_t *__restrict__ perm, float w_scale,
+                           const int32_t *__restrict__ tile_off, uint32_t *__restrict__ post, int2 *__restrict__ dir,
+                           unsigned short *__restrict__ maxw_rows, uint32_t *__restrict__ big_key,
+                           uint32_t *__restrict__ big_post, int32_t *__restrict__ big_end, int32_t *n_spilled) {
+    typedef cub::BlockScan<int, PB_THREADS> Scan;
+    __shared__ typename Scan::TempStorage scan_tmp;
+    __shared__ int64_t row_p0[PB_THREADS];
+    __shared__ int row_off[PB_THREADS];
+    extern __shared__ __align__(16) uint32_t pb_smem[];
+    uint32_t *skey = pb_smem, *spost = pb_smem + PB_CAP;
+
+    const int64_t t = blockIdx.x;
+    const int off0 = tile_off[t], n = tile_off[t + 1] - off0;
+    const bool big = n > PB_CAP;
+    if (threadIdx.x == 0) {
+        big_end[t] = big ? off0 + n : off0;
+        if (big && n_spilled) atomicAdd(n_spilled, 1);
+    }
+    uint32_t *kdst = big ? big_key + off0 : skey, *pdst = big ? big_post + off0 : spost;
+
+    // gather, PB_THREADS rows at a time: offsets by a block scan of the row lengths, then one entry per thread (its
+    // row by a binary search over the offsets: rows past the tile's end are empty and start at `total`)
+    const int64_t p0 = t * W;
+    const int nr = (int)((p0 + W < n_rows ? p0 + W : n_rows) - p0);
+    int base = 0;
+    for (int r0 = 0; r0 < nr; r0 += PB_THREADS) {
+        const int r = r0 + threadIdx.x;
+        int len = 0;
+        int64_t q = 0;
+        if (r < nr) {
+            const int64_t row = perm ? perm[p0 + r] : p0 + r;
+            q = indptr[row];
+            len = (int)(indptr[row + 1] - q);
+        }
+        int o, total;
+        Scan(scan_tmp).ExclusiveSum(len, o, total);
+        row_p0[threadIdx.x] = q;
+        row_off[threadIdx.x] = o;
+        __syncthreads();
+#pragma unroll 4
+        for (int j = threadIdx.x; j < total; j += PB_THREADS) {
+            int k = 0;          // the last row starting at or before j
+#pragma unroll
+            for (int s = PB_THREADS / 2; s; s >>= 1)
+                if (row_off[k + s] <= j) k += s;
+            const int64_t p = row_p0[k] + (j - row_off[k]);
+            kdst[base + j] = (uint32_t)indices[p];
+            pdst[base + j] = make_posting(val[p], w_scale, (uint32_t)(r0 + k));
+        }
+        base += total;
+        __syncthreads();
+    }
+    if (big) return;
+
+    // the smallest sort that holds the tile: the work of every radix pass grows with the items per thread
+    if (n <= PB_THREADS * 2) postings_sort_tile<2>(skey, spost, n, key_bits);
+    else if (n <= PB_THREADS * 4) postings_sort_tile<4>(skey, spost, n, key_bits);
+    else postings_sort_tile<PB_ITEMS>(skey, spost, n, key_bits);
+    __syncthreads();
+    for (int i = threadIdx.x; i < n; i += PB_THREADS) post[off0 + i] = spost[i];
+    postings_emit_runs(skey, spost, n, off0, t, T, Tp, dir, maxw_rows);
+}
+
+// Tiles of more than PB_CAP postings after the segmented sort of [tile_off[t], big_end[t]): keys / pst are the sorted
+// buffers (pst may be `post` itself); every other tile has an empty segment and returns.
+__global__ void __launch_bounds__(256)
+postings_big_dir_kernel(int64_t T, int64_t Tp, const int32_t *__restrict__ tile_off,
+                        const int32_t *__restrict__ big_end, const uint32_t *keys, const uint32_t *pst, uint32_t *post,
+                        int2 *__restrict__ dir, unsigned short *__restrict__ maxw_rows) {
+    const int64_t t = blockIdx.x;
+    const int off0 = tile_off[t], n = big_end[t] - off0;
+    if (n == 0) return;
+    if (pst != post)
+        for (int i = threadIdx.x; i < n; i += blockDim.x) post[off0 + i] = pst[off0 + i];
+    postings_emit_runs(keys + off0, pst + off0, n, off0, t, T, Tp, dir, maxw_rows);
 }
 
 __device__ __forceinline__ float post_w(uint32_t e) { return __half2float(__ushort_as_half((unsigned short)(e >> 16))); }
 __device__ __forceinline__ int post_c(uint32_t e) { return (int)(e & 0xffffu); }
-
-// bucket directory: one aligned 8-byte entry per (feature, tile) so that a lane fetches it in one load:
-// {int32 start, u16 length | fp16 largest |weight| << 16}
-__global__ void postings_dir_kernel(int64_t nb, const int32_t *__restrict__ ptr, const uint32_t *__restrict__ maxw,
-                                    int2 *__restrict__ dir, int64_t T, int64_t Tp,
-                                    unsigned short *__restrict__ maxw_rows) {
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= nb) return;
-    dir[i] = make_int2(ptr[i], (int)(((uint32_t)(ptr[i + 1] - ptr[i]) & 0xffffu) | (maxw[i] << 16)));
-    // the same maxima as fp16 rows of Tp tiles per feature (zero padded): what the block-max test streams
-    if (maxw_rows) maxw_rows[(i / T) * Tp + (i % T)] = (unsigned short)maxw[i];
-}
 
 __device__ __forceinline__ int dir_len(int2 d) { return d.y & 0xffff; }
 __device__ __forceinline__ float dir_maxw(int2 d) {
@@ -1220,12 +1332,25 @@ int64_t sg_num_tiles(int64_t n_right, int tile_w) {
     return t < 1 ? 1 : t;
 }
 
+// scratch of sg_postings_build: tile counts, offsets and segment ends, the segmented sort's key / posting buffers,
+// the scratch of the scan and of the segmented sort
+static size_t postings_scan_bytes(int64_t n_tiles) {
+    size_t b = 0;
+    cub::DeviceScan::ExclusiveSum(nullptr, b, (int32_t *)nullptr, (int32_t *)nullptr, n_tiles + 1);
+    return b;
+}
+static size_t postings_sort_bytes(int64_t nnz, int64_t n_cols, int64_t n_tiles) {
+    size_t b = 0;
+    cub::DoubleBuffer<uint32_t> k(nullptr, nullptr), v(nullptr, nullptr);
+    cub::DeviceSegmentedRadixSort::SortPairs(nullptr, b, k, v, (int)nnz, (int)n_tiles, (int32_t *)nullptr,
+                                             (int32_t *)nullptr, 0, bits_for((uint64_t)n_cols));
+    return b;
+}
+
 size_t sg_postings_workspace_bytes(int64_t nnz, int64_t n_cols, int64_t n_tiles) {
-    (void)nnz;
-    const int64_t nb = n_tiles * (n_cols + 1) + 1;
-    size_t b2 = 0;
-    cub::DeviceScan::ExclusiveSum(nullptr, b2, (int32_t *)nullptr, (int32_t *)nullptr, nb);
-    return 2 * align_up((size_t)nb * 4, 256) + align_up(b2, 256) + 4096;
+    return 3 * align_up((size_t)(n_tiles + 1) * 4, 256) + 3 * align_up((size_t)(nnz > 0 ? nnz : 1) * 4, 256) +
+           align_up(postings_scan_bytes(n_tiles), 256) + align_up(postings_sort_bytes(nnz, n_cols, n_tiles), 256) +
+           4096;
 }
 
 int64_t sg_num_tiles_padded(int64_t n_right, int tile_w) {
@@ -1233,8 +1358,8 @@ int64_t sg_num_tiles_padded(int64_t n_right, int tile_w) {
 }
 
 int sg_postings_build(int64_t n_rows, int64_t n_cols, int64_t nnz, const int64_t *indptr, const int32_t *indices,
-                      const float *val32, const int32_t *rank, int tile_w, int64_t indptr_base, float w_scale,
-                      int32_t *bucket_ptr, void *bucket_dir, void *bucket_maxw, void *postings, void *ws,
+                      const float *val32, const int32_t *perm, int tile_w, int64_t indptr_base, float w_scale,
+                      void *bucket_dir, void *bucket_maxw, void *postings, int32_t *n_spilled, void *ws,
                       size_t ws_bytes, void *stream_) {
     cudaStream_t st = (cudaStream_t)stream_;
     (void)indptr_base;      // indptr holds absolute positions into indices / val32
@@ -1242,39 +1367,45 @@ int sg_postings_build(int64_t n_rows, int64_t n_cols, int64_t nnz, const int64_t
         return fail(SG_ERR_INVALID, "tile_w must be a multiple of 32 up to 32768 (16-bit bucket lengths)");
     if (nnz >= (int64_t)0x7fffffff)
         return fail(SG_ERR_OVERFLOW, "right matrix nnz %lld does not fit int32 postings", (long long)nnz);
+    if (!bucket_dir || !bucket_maxw || !postings) return fail(SG_ERR_INVALID, "postings outputs must not be NULL");
     const int64_t T = sg_num_tiles(n_rows, tile_w);
+    const int64_t Tp = sg_num_tiles_padded(n_rows, tile_w);
     const int64_t V1 = n_cols + 1;
-    const int64_t nb = T * V1 + 1;
-    if (nb >= (int64_t)0x7fffffff) return fail(SG_ERR_OVERFLOW, "bucket table %lld too large", (long long)nb);
+    if (T * V1 >= (int64_t)0x7fffffff) return fail(SG_ERR_OVERFLOW, "bucket table %lld too large", (long long)(T * V1));
+    const int key_bits = bits_for((uint64_t)n_cols);
     Arena ar(ws, ws_bytes);
-    int32_t *cnt = ar.take<int32_t>((size_t)nb);
-    uint32_t *maxw = ar.take<uint32_t>((size_t)nb);
-    size_t cub_bytes = 0;
-    cub::DeviceScan::ExclusiveSum(nullptr, cub_bytes, cnt, bucket_ptr, nb);
-    char *tmp = ar.take<char>(cub_bytes);
+    int32_t *tile_cnt = ar.take<int32_t>((size_t)T + 1);
+    int32_t *tile_off = ar.take<int32_t>((size_t)T + 1);
+    int32_t *big_end = ar.take<int32_t>((size_t)T + 1);
+    const size_t n_buf = (size_t)(nnz > 0 ? nnz : 1);
+    uint32_t *big_key = ar.take<uint32_t>(n_buf), *big_key2 = ar.take<uint32_t>(n_buf);
+    uint32_t *big_post = ar.take<uint32_t>(n_buf);
+    size_t scan_bytes = postings_scan_bytes(T), sort_bytes = postings_sort_bytes(nnz, n_cols, T);
+    char *scan_tmp = ar.take<char>(scan_bytes), *sort_tmp = ar.take<char>(sort_bytes);
     if (!ar.ok()) return fail(SG_ERR_INVALID, "postings workspace too small (%zu < %zu)", ws_bytes, ar.off);
-    SG_CUDA_TRY(cudaMemsetAsync(cnt, 0, (size_t)nb * 4, st));
-    SG_CUDA_TRY(cudaMemsetAsync(maxw, 0, (size_t)nb * 4, st));
-    const unsigned row_grid = (unsigned)((n_rows + 7) / 8);
-    if (n_rows > 0 && nnz > 0) {
-        postings_count_kernel<<<row_grid, 256, 0, st>>>(n_rows, indptr, indices, val32, rank, tile_w, T, w_scale, cnt,
-                                                        maxw);
-        SG_LAUNCH_CHECK();
-    }
-    SG_CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, cub_bytes, cnt, bucket_ptr, nb, st));
-    if (bucket_dir) {
-        const int64_t Tp = sg_num_tiles_padded(n_rows, tile_w);
-        if (bucket_maxw) SG_CUDA_TRY(cudaMemsetAsync(bucket_maxw, 0, (size_t)(V1 * Tp) * 2, st));
-        postings_dir_kernel<<<(unsigned)((nb - 1 + 255) / 256), 256, 0, st>>>(nb - 1, bucket_ptr, maxw,
-                                                                              (int2 *)bucket_dir, T, Tp,
-                                                                              (unsigned short *)bucket_maxw);
-        SG_LAUNCH_CHECK();
-    }
-    if (n_rows > 0 && nnz > 0) {
-        postings_scatter_kernel<<<row_grid, 256, 0, st>>>(n_rows, indptr, indices, val32, rank, tile_w, T, w_scale,
-                                                          bucket_ptr, cnt, (uint32_t *)postings);
-        SG_LAUNCH_CHECK();
-    }
+
+    // empty buckets and the padding tiles up to Tp stay zero
+    SG_CUDA_TRY(cudaMemsetAsync(bucket_dir, 0, (size_t)(T * V1) * 8, st));
+    SG_CUDA_TRY(cudaMemsetAsync(bucket_maxw, 0, (size_t)(V1 * Tp) * 2, st));
+    if (n_rows <= 0 || nnz <= 0) return SG_OK;
+    postings_tile_count_kernel<<<(unsigned)((T + 1 + 7) / 8), 256, 0, st>>>(n_rows, T, tile_w, indptr, perm,
+                                                                            tile_cnt);
+    SG_LAUNCH_CHECK();
+    SG_CUDA_TRY(cub::DeviceScan::ExclusiveSum(scan_tmp, scan_bytes, tile_cnt, tile_off, T + 1, st));
+    SG_CUDA_TRY(cudaFuncSetAttribute(postings_tile_build_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)PB_SMEM));
+    postings_tile_build_kernel<<<(unsigned)T, PB_THREADS, PB_SMEM, st>>>(
+        n_rows, T, Tp, tile_w, key_bits, indptr, indices, val32, perm, w_scale, tile_off, (uint32_t *)postings,
+        (int2 *)bucket_dir, (unsigned short *)bucket_maxw, big_key, big_post, big_end, n_spilled);
+    SG_LAUNCH_CHECK();
+    // tiles of more than PB_CAP postings: sorted in global memory; the other segments are empty
+    cub::DoubleBuffer<uint32_t> keys(big_key, big_key2), vals(big_post, (uint32_t *)postings);
+    SG_CUDA_TRY(cub::DeviceSegmentedRadixSort::SortPairs(sort_tmp, sort_bytes, keys, vals, (int)nnz, (int)T, tile_off,
+                                                         big_end, 0, key_bits, st));
+    postings_big_dir_kernel<<<(unsigned)T, 256, 0, st>>>(T, Tp, tile_off, big_end, keys.Current(), vals.Current(),
+                                                         (uint32_t *)postings, (int2 *)bucket_dir,
+                                                         (unsigned short *)bucket_maxw);
+    SG_LAUNCH_CHECK();
     return SG_OK;
 }
 
