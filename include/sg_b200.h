@@ -279,6 +279,8 @@ int sg_tile_bounds(int64_t n_right, const int32_t *perm /*[dev] position -> row,
  * unordered pair {i, j} is reported once (the pair (i, i) too); sg_rescore's `mirror_count` restores the other half.
  * `group_items` [dev] sg_num_tiles()/tiles_per_group + 1 entries (rounded up) is scratch for the work items of the
  * triangle, required with diag_rank.
+ * Block-max test: a (row, column tile) pair is walked only if sum_f |a_f| * max|w_(f,t)| over ALL the row's kept
+ * features (bucket_maxw, fp16, rounded up) can reach the pair's threshold.
  */
 #define SG_ACC_F32 0
 #define SG_ACC_U16 1 /* 1/32768 fixed point: caller adds 2e-5 per kept feature to the margin; weights >= 0, scores < 2 */
@@ -316,9 +318,8 @@ int sg_cossim_candidates(const int64_t *a_indptr /*[dev]*/, const int32_t *a_len
  * Self-match (`self_rank` [dev] per row id: the row's position in the common processing order, perm_a the same
  * order): `flags` & SG_FLOOR_SEED walks only the column-tile group holding the row, starting at the 64-tile batch that
  * holds it; without it every other group.  self_rank = NULL: every group (two matrices).
- * `flags` & SG_FLOOR_LONG_ROWS (acc_dtype SG_ACC_F32 only): rows with more than 32 kept features are bounded by the
- * block-max test over all their features too, instead of walking every tile (the no-threshold mode of the top-n
- * product, where long rows keep all their features).
+ * `flags` & SG_FLOOR_LONG_ROWS is accepted and changes nothing: every candidates kernel bounds rows of more than 32
+ * kept features by the block-max test over all their features.
  */
 #define SG_FLOOR_SEED 1
 #define SG_FLOOR_LONG_ROWS 2

@@ -967,6 +967,9 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
         stats["prune"], stats["acc"] = prune, acc
         stats["kernel"] = "tiles" if use_tiles else "row"
         stats["n_candidates_estimate"] = est
+        kept_len = (l_len[row_begin:row_end] if l_len is not None else
+                    A.d_indptr[row_begin + 1:row_end + 1] - A.d_indptr[row_begin:row_end])
+        stats["n_rows_long"] = int((kept_len > 32).sum().item())     # bounded over all their kept features
         if stats.get("count_macs") and l_len is not None:
             df = feature_df(B).long()
             pos = t.arange(A.d_indices.numel(), device=dev)
@@ -1180,9 +1183,9 @@ def _cossim_topn_floor(A, B, top_n, threshold, row_begin, row_end, tile_w, stats
     floor is taken only if the sampled candidate count of the usual path needs more than a quarter of device memory;
     otherwise None is returned and the caller runs the usual path.
 
-    threshold <= 0 (no threshold): the floors start from topn_floor_init, the left rows are pruned against them
-    before the first launch, and the candidates kernel bounds rows of more than 32 kept features by the block-max test
-    as well (SG_FLOOR_LONG_ROWS); the accumulator is fp32.
+    threshold <= 0 (no threshold): the floors start from topn_floor_init and the left rows are pruned against them
+    before the first launch; the accumulator is fp32.  Long rows (more than 32 kept features, which a name keeps
+    without a threshold) are bounded by the block-max test like every other row.
 
     `row_best` (cossim_nearest, top_n = 1): the arg-max re-score with the floor replaces the top-n selection.  Every
     pair scoring at least the floor is re-scored, so all pairs tied at a row's best are among them."""
@@ -1272,7 +1275,6 @@ def _cossim_topn_floor(A, B, top_n, threshold, row_begin, row_end, tile_w, stats
         mark(stats, "floor_init")
     else:
         floor_buf = t.zeros(n_left, dtype=t.float32, device=dev)
-    flags = _lib.SG_FLOOR_LONG_ROWS if no_threshold else 0
 
     def launch(perm, n, arrs, row_buf, col_buf, part_buf, capacity, seed):
         l_idx, l_val, l_len, l_thr, l_xp, _ = arrs
@@ -1282,7 +1284,7 @@ def _cossim_topn_floor(A, B, top_n, threshold, row_begin, row_end, tile_w, stats
             A.shape[1], _ptr(bucket_dir), _ptr(bucket_maxw), _ptr(post), _ptr(perm_b), tile_w, acc_code,
             max(B.norm_bound, 1.0), thr_c, _ptr(l_thr), _ptr(l_xp), _ptr(tile_bound), tiles_per_group, _ptr(row_buf),
             _ptr(col_buf), _ptr(part_buf), capacity, c_count, c_queue, warps, _ptr(floor_buf), top_n, margin,
-            margin_pf, _ptr(self_rank), flags | (_lib.SG_FLOOR_SEED if seed else 0), _stream()))
+            margin_pf, _ptr(self_rank), _lib.SG_FLOOR_SEED if seed else 0, _stream()))
         LAUNCH_COUNTS["candidates"] += 1
         return int(counters[0].item())
 
@@ -1405,7 +1407,7 @@ def _cossim_topn_floor(A, B, top_n, threshold, row_begin, row_end, tile_w, stats
             l_len = arrays[2]
             kept = (l_len[row_begin:row_end] if l_len is not None else
                     A.d_indptr[row_begin + 1:row_end + 1] - A.d_indptr[row_begin:row_end])
-            stats["n_rows_long"] = int((kept > 32).sum().item())      # bounded by SG_FLOOR_LONG_ROWS
+            stats["n_rows_long"] = int((kept > 32).sum().item())      # bounded over all their kept features
         stats["prune"], stats["acc"], stats["kernel"] = (floor_level if no_threshold else level), acc, "row"
         stats["n_candidates_estimate"] = est
         stats["n_candidates_seed"], stats["n_candidates_main"] = n_seed, n_main

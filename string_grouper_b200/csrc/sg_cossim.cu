@@ -389,11 +389,9 @@ __device__ __forceinline__ void apply_buckets(AccT *__restrict__ acc, const uint
 // column-tile group, starting at the 64-tile batch that holds the row (clusters of identical names sit next to each
 // other in that order, so this is where floors rise first); `seed` = 0 walks every other group.
 //
-// Long rows (LONG_ROWS, cossim_candidates_floor_long_kernel): the usual kernel walks every tile of a row with more than
-// 32 kept features, because only the first 32 stay in registers for the block-max bound.  That is cheap at a high
-// threshold, where pruning leaves few such rows, but not without a threshold, where a long name keeps all its
-// features.  This variant bounds them too: ub(t) over ALL kept features, 32 at a time, the later chunks' {feature,
-// weight} loaded once per 64-tile batch, with the same fp16 round-up and a slack of 5e-4 per feature.  Every hfma2
+// Long rows (more than 32 kept features: long records rows, names without a threshold): only the first 32 stay in
+// registers, but ub(t) is taken over ALL kept features, the later ones 32 at a time, their {feature, weight} loaded
+// once per 64-tile batch, with the same fp16 round-up and a slack of 5e-4 per feature.  Every hfma2
 // rounds once; while the running sum stays below 2 (ulp 2^-10) that is at most 2^-11 < 5e-4, and once it reaches 2
 // it stays there (non-negative terms, monotone rounding), above any threshold of scores in [0, 1].
 struct FloorArgs {
@@ -422,7 +420,7 @@ __device__ __forceinline__ void floor_merge(float &kept, float x, int lane) {
     }
 }
 
-template <int NW, typename AccT, bool FLOOR, bool LONG_ROWS = false, bool RANGE = false>
+template <int NW, typename AccT, bool FLOOR, bool RANGE = false>
 __device__ __forceinline__ void
 candidates_body(const int64_t *__restrict__ a_indptr, const int32_t *__restrict__ a_len,
                 const int32_t *__restrict__ a_idx, const float *__restrict__ a_val, int64_t row_begin,
@@ -524,7 +522,7 @@ candidates_body(const int64_t *__restrict__ a_indptr, const int32_t *__restrict_
         const int2 *drow = bdir + f0 * n_tiles;
         const int nk = nf < 32 ? nf : 32;
         // fp16 arithmetic of the bound: one rounding of at most 2^-11 (values below 2) per kept feature
-        const float slack = 5e-4f * (float)(LONG_ROWS ? nf : nk) + 1e-4f;
+        const float slack = 5e-4f * (float)nf + 1e-4f;
 
         for (int tb0 = tb_begin; tb0 < t_end; tb0 += 64) {
             int tb = tb0;
@@ -541,7 +539,7 @@ candidates_body(const int64_t *__restrict__ a_indptr, const int32_t *__restrict_
             unsigned m_even, m_odd;
             const int t0 = tb + 2 * lane;
             const bool up0 = (t0 + 1) * W > dr, up1 = (t0 + 2) * W > dr;
-            if (LONG_ROWS || nf <= 32) {
+            {
                 __half2 ub2 = __float2half2_rn(0.f);
                 const uint32_t *mrow = maxw_h + (tb >> 1) + lane;
                 // SG_FILTER_MLP block-maxima loads in flight per lane
@@ -559,22 +557,20 @@ candidates_body(const int64_t *__restrict__ a_indptr, const int32_t *__restrict_
                     for (int u = 0; u < SG_FILTER_MLP; ++u)
                         ub2 = __hfma2(ak2[u], *reinterpret_cast<const __half2 *>(&m[u]), ub2);
                 }
-                if constexpr (LONG_ROWS) {
-                    // the kept features after the first 32, one chunk of 32 at a time
-                    for (int base = 32; base < nf; base += 32) {
-                        int fl = 0;
-                        __half2 al = __float2half2_rn(0.f);
-                        if (base + lane < nf) {
-                            fl = a_idx[p0 + base + lane];
-                            al = __half2half2(__float2half_ru(fabsf(a_val[p0 + base + lane] * a_scale)));
-                        }
-                        const int nc = nf - base < 32 ? nf - base : 32;
-                        for (int kk = 0; kk < nc; ++kk) {
-                            const int fk = __shfl_sync(FULL, fl, kk);
-                            const __half2 ak = __shfl_sync(FULL, al, kk);
-                            const uint32_t mv = mrow[fk * (Tp >> 1)];
-                            ub2 = __hfma2(ak, *reinterpret_cast<const __half2 *>(&mv), ub2);
-                        }
+                // the kept features after the first 32, one chunk of 32 at a time
+                for (int base = 32; base < nf; base += 32) {
+                    int fl = 0;
+                    __half2 al = __float2half2_rn(0.f);
+                    if (base + lane < nf) {
+                        fl = a_idx[p0 + base + lane];
+                        al = __half2half2(__float2half_ru(fabsf(a_val[p0 + base + lane] * a_scale)));
+                    }
+                    const int nc = nf - base < 32 ? nf - base : 32;
+                    for (int kk = 0; kk < nc; ++kk) {
+                        const int fk = __shfl_sync(FULL, fl, kk);
+                        const __half2 ak = __shfl_sync(FULL, al, kk);
+                        const uint32_t mv = mrow[fk * (Tp >> 1)];
+                        ub2 = __hfma2(ak, *reinterpret_cast<const __half2 *>(&mv), ub2);
                     }
                 }
                 const float2 ub = __half22float2(ub2);
@@ -583,9 +579,6 @@ candidates_body(const int64_t *__restrict__ a_indptr, const int32_t *__restrict_
                 const float thr1 = xp > 0.f ? fmaxf(fmaf(-xp, tb2.y, thr_r), 0.f) : thr_r;
                 m_even = __ballot_sync(FULL, t0 < t_end && up0 && ub.x + slack > thr0);
                 m_odd = __ballot_sync(FULL, t0 + 1 < t_end && up1 && ub.y + slack > thr1);
-            } else {        // rows with more than 32 kept features: every tile is walked
-                m_even = __ballot_sync(FULL, t0 < t_end && up0);
-                m_odd = __ballot_sync(FULL, t0 + 1 < t_end && up1);
             }
             // ---- walk the surviving tiles; the directory entry of the next one is fetched ahead
             int t = -1;
@@ -717,14 +710,8 @@ __global__ void __launch_bounds__(NW * 32, min_ctas(NW)) cossim_candidates_floor
 
 template <int NW, typename AccT>
 __global__ void __launch_bounds__(NW * 32, min_ctas(NW))
-    cossim_candidates_floor_long_kernel(SG_CAND_PARAMS, FloorArgs fa) {
-    candidates_body<NW, AccT, true, true>(SG_CAND_ARGS, fa);
-}
-
-template <int NW, typename AccT>
-__global__ void __launch_bounds__(NW * 32, min_ctas(NW))
     cossim_candidates_range_kernel(SG_CAND_PARAMS, const int32_t *__restrict__ hi_pos) {
-    candidates_body<NW, AccT, false, false, true>(SG_CAND_ARGS, FloorArgs{}, hi_pos);
+    candidates_body<NW, AccT, false, true>(SG_CAND_ARGS, FloorArgs{}, hi_pos);
 }
 #undef SG_CAND_PARAMS
 #undef SG_CAND_ARGS
@@ -1411,7 +1398,7 @@ int sg_postings_build(int64_t n_rows, int64_t n_cols, int64_t nnz, const int64_t
 
 }  // extern "C"
 
-template <int NW, typename AccT, bool FLOOR, bool LONG_ROWS = false, bool RANGE = false>
+template <int NW, typename AccT, bool FLOOR, bool RANGE = false>
 static int launch_candidates(const int64_t *a_indptr, const int32_t *a_len, const int32_t *a_indices,
                              const float *a_val32, int64_t row_begin, int64_t row_end, const int32_t *perm_a,
                              int64_t n_right, int64_t n_cols, const void *bucket_dir, const void *bucket_maxw,
@@ -1425,7 +1412,6 @@ static int launch_candidates(const int64_t *a_indptr, const int32_t *a_len, cons
     const size_t smem = (size_t)NW * tile_w * sizeof(AccT);
     const void *kern;
     if constexpr (RANGE) kern = (const void *)cossim_candidates_range_kernel<NW, AccT>;
-    else if constexpr (LONG_ROWS) kern = (const void *)cossim_candidates_floor_long_kernel<NW, AccT>;
     else if constexpr (FLOOR) kern = (const void *)cossim_candidates_floor_kernel<NW, AccT>;
     else kern = (const void *)cossim_candidates_kernel<NW, AccT>;
     SG_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -1463,8 +1449,6 @@ static int launch_candidates(const int64_t *a_indptr, const int32_t *a_len, cons
         row_queue
     if constexpr (RANGE)
         cossim_candidates_range_kernel<NW, AccT><<<(unsigned)ctas, NW * 32, smem, st>>>(SG_KARGS, hi_pos);
-    else if constexpr (LONG_ROWS)
-        cossim_candidates_floor_long_kernel<NW, AccT><<<(unsigned)ctas, NW * 32, smem, st>>>(SG_KARGS, fa);
     else if constexpr (FLOOR)
         cossim_candidates_floor_kernel<NW, AccT><<<(unsigned)ctas, NW * 32, smem, st>>>(SG_KARGS, fa);
     else
@@ -1474,8 +1458,7 @@ static int launch_candidates(const int64_t *a_indptr, const int32_t *a_len, cons
     return SG_OK;
 }
 
-// fa == NULL: cossim_candidates_kernel, or with `hi_pos` the position-range variant; otherwise the floor variant (with
-// `long_rows` the one that also bounds rows of more than 32 kept features)
+// fa == NULL: cossim_candidates_kernel, or with `hi_pos` the position-range variant; otherwise the floor variant
 static int cossim_candidates(const int64_t *a_indptr, const int32_t *a_len, const int32_t *a_indices,
                              const float *a_val32, int64_t row_begin, int64_t row_end, const int32_t *perm_a,
                              int64_t n_right, int64_t n_cols, const void *bucket_dir, const void *bucket_maxw,
@@ -1485,8 +1468,7 @@ static int cossim_candidates(const int64_t *a_indptr, const int32_t *a_len, cons
                              int64_t tiles_per_group, const int32_t *diag_rank, unsigned long long *group_items,
                              int32_t *cand_row, int32_t *cand_col, float *cand_partial, int64_t cand_cap,
                              unsigned long long *cand_count, unsigned long long *row_queue, int warps_per_cta,
-                             void *stream_, const FloorArgs *fa, bool long_rows = false,
-                             const int32_t *hi_pos = nullptr) {
+                             void *stream_, const FloorArgs *fa, const int32_t *hi_pos = nullptr) {
     cudaStream_t st = (cudaStream_t)stream_;
     if (row_end <= row_begin || n_right <= 0) return SG_OK;
     if (acc_dtype != SG_ACC_F32 && acc_dtype != SG_ACC_U16)
@@ -1515,17 +1497,12 @@ static int cossim_candidates(const int64_t *a_indptr, const int32_t *a_len, cons
         // the range variant is built for the default 8 warps only
         if (warps_per_cta != 8) return fail(SG_ERR_INVALID, "the position-range variant runs with 8 warps per CTA");
         if (!diag_rank || !group_items) return fail(SG_ERR_INVALID, "the position range needs lo_pos and group_items");
-        return acc_dtype == SG_ACC_U16 ? launch_candidates<8, uint16_t, false, false, true>(SG_ARGS, FloorArgs{}, hi_pos)
-                                       : launch_candidates<8, float, false, false, true>(SG_ARGS, FloorArgs{}, hi_pos);
+        return acc_dtype == SG_ACC_U16 ? launch_candidates<8, uint16_t, false, true>(SG_ARGS, FloorArgs{}, hi_pos)
+                                       : launch_candidates<8, float, false, true>(SG_ARGS, FloorArgs{}, hi_pos);
     }
     if (fa) {
         // the floor variant is built for the default 8 warps only
         if (warps_per_cta != 8) return fail(SG_ERR_INVALID, "the top-n floor variant runs with 8 warps per CTA");
-        if (long_rows) {        // built for the fp32 accumulator only: no threshold means near-zero candidate thresholds
-            if (acc_dtype != SG_ACC_F32)
-                return fail(SG_ERR_INVALID, "SG_FLOOR_LONG_ROWS runs with the fp32 accumulator (SG_ACC_F32)");
-            return launch_candidates<8, float, true, true>(SG_ARGS, *fa);
-        }
         return acc_dtype == SG_ACC_U16 ? launch_candidates<8, uint16_t, true>(SG_ARGS, *fa)
                                        : launch_candidates<8, float, true>(SG_ARGS, *fa);
     }
@@ -1588,7 +1565,7 @@ int sg_cossim_candidates_floor(const int64_t *a_indptr, const int32_t *a_len, co
                              bucket_dir, bucket_maxw, postings, perm_b, tile_w, acc_dtype, a_scale, cand_threshold,
                              cand_threshold_row, pruned_norm_row, tile_bound, tiles_per_group, nullptr, nullptr,
                              cand_row, cand_col, cand_partial, cand_cap, cand_count, row_queue, warps_per_cta, stream_,
-                             &fa, (flags & SG_FLOOR_LONG_ROWS) != 0);
+                             &fa);
 }
 
 int sg_cossim_candidates_range(const int64_t *a_indptr, const int32_t *a_len, const int32_t *a_indices,
@@ -1606,7 +1583,7 @@ int sg_cossim_candidates_range(const int64_t *a_indptr, const int32_t *a_len, co
                              bucket_dir, bucket_maxw, postings, perm_b, tile_w, acc_dtype, a_scale, cand_threshold,
                              cand_threshold_row, pruned_norm_row, tile_bound, tiles_per_group, lo_pos, group_items,
                              cand_row, cand_col, cand_partial, cand_cap, cand_count, row_queue, warps_per_cta, stream_,
-                             nullptr, false, hi_pos);
+                             nullptr, hi_pos);
 }
 
 }  // extern "C"
