@@ -660,6 +660,18 @@ int sg_group_reps(int64_t n, int64_t nnz, const int32_t *row, const int32_t *col
                   int centroid, int32_t *rep /*[dev] n*/, void *ws, size_t ws_bytes, void *stream);
 
 /* ------------------------------------------------------------------------- *
+ * Star groups (group_similar_strings(linkage='star'), csrc/sg_star.cu): greedy star clustering of the match graph.
+ * Strings are ranked by index (centroid = 0) or by the similarity sum of sg_group_reps descending, then index
+ * (centroid = 1).  In rank order, a string not yet assigned becomes a pivot and takes every unassigned neighbour
+ * (u ~ v when (u, v) or (v, u) is stored); rep[i] = the pivot of i's group, so rep[i] is i or one of i's matches.
+ * Input: the match list sorted by row (any column order, symmetric or not).  Computed in rounds with the serial
+ * rule's result, as many as needed (no cap); the stream is synchronised once every 8 rounds.
+ * ------------------------------------------------------------------------- */
+size_t sg_group_star_workspace_bytes(int64_t n);
+int sg_group_star(int64_t n, int64_t nnz, const int32_t *row, const int32_t *col, const double *score,
+                  int centroid, int32_t *rep /*[dev] n*/, void *ws, size_t ws_bytes, void *stream);
+
+/* ------------------------------------------------------------------------- *
  * Nearest master per duplicate (SURVEY.md §8f row 3).  Replaces the reduction of StringGrouper._get_nearest_matches
  * (sg.py:783-849; the groupby / idxmax of :803-807): best[j] = left row with the highest similarity to right row j,
  * the smallest left index among equal scores, -1 when no match holds j.  Input: the match list in any order.

@@ -1544,6 +1544,23 @@ def group_reps(M, n, centroid, keep_device=False):
     return (host, rep) if keep_device else host
 
 
+def group_star(M, n, centroid, keep_device=False):
+    """Pivot of every string's star group (group_similar_strings(linkage='star'), csrc/sg_star.cu) from the
+    row-sorted device match list: strings ranked by index, or by group_reps' similarity sum descending (centroid), each
+    unassigned string in rank order takes its unassigned neighbours.  keep_device: also return the int32 device tensor."""
+    t = require_cuda()
+    L = _lib.load()
+    dev = M.d_row.device
+    rep = _empty(n, t.int32, dev)
+    ws_bytes = int(L.sg_group_star_workspace_bytes(n))
+    ws = _empty(ws_bytes, t.uint8, dev)
+    _lib.check(L.sg_group_star(n, M.nnz, _ptr(M.d_row), _ptr(M.d_col), _ptr(M.d_score), 1 if centroid else 0,
+                               _ptr(rep), _ptr(ws), ws_bytes, _stream()))
+    LAUNCH_COUNTS["groups"] += 7 if centroid else 3
+    host = rep[:n].cpu().numpy().astype(np.int64)
+    return (host, rep) if keep_device else host
+
+
 def nearest_master(M, n_right):
     """int64 [n_right]: for every right row the left row of its best match (smallest index among equal scores),
     -1 without a match — the reduction of StringGrouper._get_nearest_matches (string_grouper.py:803-807)."""

@@ -122,6 +122,8 @@ SIGNATURES = {
     "sg_symmetrize": (_i32, [_i64, _i64, _i32, _p, _p, _p, _p, _p, _p, _p, _p, _sz, _p]),
     "sg_group_reps_workspace_bytes": (_sz, [_i64]),
     "sg_group_reps": (_i32, [_i64, _i64, _p, _p, _p, _i32, _p, _p, _sz, _p]),
+    "sg_group_star_workspace_bytes": (_sz, [_i64]),
+    "sg_group_star": (_i32, [_i64, _i64, _p, _p, _p, _i32, _p, _p, _sz, _p]),
     "sg_nearest_master_workspace_bytes": (_sz, [_i64]),
     "sg_nearest_master": (_i32, [_i64, _p, _p, _p, _i64, _p, _p, _sz, _p]),
     "sg_gather_workspace_bytes": (_sz, [_i64]),

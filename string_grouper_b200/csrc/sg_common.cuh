@@ -56,4 +56,9 @@ __device__ __forceinline__ int lane_id() { return threadIdx.x & 31; }
 // zeroed here), workspace of sg_tfidf_transform_workspace_bytes
 int transform_indptr(int64_t n_docs, int32_t *row_nnz, int64_t *indptr, void *ws, size_t ws_bytes, cudaStream_t st);
 
+// sg_groups.cu: weight[i] = row i's similarity sum exactly as the 'centroid' representative uses it (row-sorted list);
+// label and best are n-element scratch
+int group_row_weights(int64_t n, int64_t nnz, const int32_t *row, const double *score, int32_t *label, double *weight,
+                      unsigned long long *best, cudaStream_t st);
+
 }  // namespace sg

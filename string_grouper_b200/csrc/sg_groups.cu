@@ -140,6 +140,18 @@ __global__ void nearest_finish_kernel(int64_t n, int32_t *__restrict__ best_row)
     if (i < n && best_row[i] == 0x7f7f7f7f) best_row[i] = -1;      // the byte-wise 0x7f fill = "no row yet"
 }
 
+// weight[i] = the 'centroid' similarity sum of row i, from the kernel sg_group_reps uses (same bits).  label and best
+// are n-element scratch: every row is its own label, so the per-label maximum is not contended.
+int group_row_weights(int64_t n, int64_t nnz, const int32_t *row, const double *score, int32_t *label, double *weight,
+                      unsigned long long *best, cudaStream_t st) {
+    const unsigned gn = (unsigned)((n + 255) / 256);
+    cc_init_kernel<<<gn, 256, 0, st>>>(n, label);
+    SG_LAUNCH_CHECK();
+    cc_rowsum_kernel<<<gn, 256, 0, st>>>(n, nnz, row, score, label, weight, best);
+    SG_LAUNCH_CHECK();
+    return SG_OK;
+}
+
 }  // namespace sg
 
 using namespace sg;

@@ -18,7 +18,7 @@ import numpy as np
 import pandas as pd
 
 from . import _device, _dist, _ingest, _lib
-from .string_grouper import (DEFAULT_ID_NAME, GROUP_REP_CENTROID, GROUP_REP_PREFIX, LEFT_PREFIX, RIGHT_PREFIX,
+from .string_grouper import (DEFAULT_ID_NAME, GROUP_REP_PREFIX, LEFT_PREFIX, RIGHT_PREFIX,
                              StringGrouper, _side_columns, validate_is_fit)
 
 SIMILARITY_PREFIX = 'similarity_'
@@ -196,12 +196,7 @@ class _RecordsGrouper(StringGrouper):
         return pd.DataFrame(dict(flat), copy=False)
 
     def _deduplicate(self, ignore_index=False) -> pd.DataFrame:
-        n = len(self._master)
-        centroid = self._config.group_rep == GROUP_REP_CENTROID
-        if self._matches_device is not None:
-            rep = _device.group_reps(self._matches_device, n, centroid)
-        else:
-            rep = self._host_group_reps(n, centroid)
+        rep = self._representatives(len(self._master))
         records = self._frames[0]
         output = records[self._fields].iloc[rep].reset_index(drop=ignore_index)
         output.columns = [f'{GROUP_REP_PREFIX}{c}' for c in output.columns]

@@ -41,6 +41,9 @@ DEFAULT_INCLUDE_ZEROES: bool = True
 GROUP_REP_CENTROID: str = 'centroid'
 GROUP_REP_FIRST: str = 'first'
 DEFAULT_GROUP_REP: str = GROUP_REP_CENTROID
+LINKAGE_SINGLE: str = 'single'
+LINKAGE_STAR: str = 'star'
+DEFAULT_LINKAGE: str = LINKAGE_SINGLE
 DEFAULT_FORCE_SYMMETRIES: bool = True
 DEFAULT_N_BLOCKS: Optional[Tuple[int, int]] = None
 DEFAULT_NORMALIZE_TO_ASCII: bool = True
@@ -61,6 +64,12 @@ class StringGrouperConfig(NamedTuple):
     `number_of_processes` is accepted for compatibility and ignored (the product runs on the GPU);
     `n_blocks` is validated like the reference, but the result does not depend on it (the kernel picks
     its own column tiles; the reference's own tests pin this invariance, ref test file :191-336).
+
+    `linkage` (not in the reference) decides the groups of a self-match's get_groups(): 'single' (default, the
+    reference's rule) groups the connected components of the match graph, so chains A ~ B ~ C join A and C however
+    unlike they are; 'star' visits the strings in group_rep order (by index for 'first', by similarity sum descending
+    for 'centroid') and makes each string not yet grouped the representative of its ungrouped matches, so every
+    string is its representative or matched to it directly.  Where every component is a clique both give one frame.
     """
     ngram_size: int = DEFAULT_NGRAM_SIZE
     tfidf_matrix_dtype: type = DEFAULT_TFIDF_MATRIX_DTYPE
@@ -76,6 +85,7 @@ class StringGrouperConfig(NamedTuple):
     force_symmetries: bool = DEFAULT_FORCE_SYMMETRIES
     n_blocks: Optional[Tuple[int, int]] = DEFAULT_N_BLOCKS
     normalize_to_ascii: bool = DEFAULT_NORMALIZE_TO_ASCII
+    linkage: str = DEFAULT_LINKAGE
 
 
 class StringGrouperNotFitException(Exception):
@@ -627,21 +637,16 @@ class StringGrouper(object):
         return out.squeeze(axis=1)
 
     def _deduplicate(self, ignore_index=False) -> Union[pd.DataFrame, pd.Series]:
-        """Connected components of the match graph, one representative per group (ref:851-904)."""
+        """One representative per group (ref:851-904): connected components of the match graph (linkage='single'),
+        or star groups around pivots (linkage='star')."""
         n = len(self._master)
-        centroid = self._config.group_rep == GROUP_REP_CENTROID
         rep_values = None
-        if self._matches_device is not None:
-            # components, similarity sums and representatives on the device (csrc/sg_groups.cu)
-            rep, d_rep = _device.group_reps(self._matches_device, n, centroid, keep_device=True)
-            raw = self._raw_device
-            if raw is not None and n > 0 and _is_arrow_str(self._master) and raw.n_master == n:
-                # the strings are in HBM too: gather the representatives there (the Series.iloc of ref:897)
-                (rhost,) = _device.gather_strings(raw, [(0, d_rep, n)])
-                rep_values = _gathered_array(self._master, *rhost)
-        else:
-            # the list was edited by add_match / remove_match: host statement of the same rule
-            rep = self._host_group_reps(n, centroid)
+        rep, d_rep = self._representatives(n, keep_device=True)
+        raw = self._raw_device
+        if d_rep is not None and raw is not None and n > 0 and _is_arrow_str(self._master) and raw.n_master == n:
+            # the strings are in HBM too: gather the representatives there (the Series.iloc of ref:897)
+            (rhost,) = _device.gather_strings(raw, [(0, d_rep, n)])
+            rep_values = _gathered_array(self._master, *rhost)
 
         prefix = GROUP_REP_PREFIX
         label = f'{prefix}{self._master.name}' if self._master.name else prefix[:-1]
@@ -674,8 +679,7 @@ class StringGrouper(object):
         graph = csr_matrix((np.full(len(pairs), 1), (rows, cols)), shape=(n, n))
         _, group = connected_components(csgraph=graph, directed=True)
         if centroid:
-            graph.data = pairs['similarity'].to_numpy()
-            weight = np.asarray(graph.sum(axis=1)).squeeze(axis=1)
+            weight = _centroid_weight(graph, pairs)
             order = np.lexsort((np.arange(n), -weight, group))   # per group: weight desc, first index on ties
         else:
             order = np.lexsort((np.arange(n), group))            # per group: first index
@@ -684,6 +688,30 @@ class StringGrouper(object):
         rep_of_group = np.empty(group.max() + 1 if n else 0, dtype=np.int64)
         rep_of_group[group[order][head]] = order[head]
         return rep_of_group[group]
+
+    def _host_star_reps(self, n, centroid):
+        """Pivot of every string's star group from the host match list: the rule of csrc/sg_star.cu, ranked by the
+        similarity sum of _host_group_reps (centroid) or by index."""
+        pairs = self._matches_list
+        rows, cols = pairs.master_side.to_numpy(), pairs.dupe_side.to_numpy()
+        weight = None
+        if centroid:
+            weight = _centroid_weight(csr_matrix((np.full(len(pairs), 1), (rows, cols)), shape=(n, n)), pairs)
+        return star_representatives(n, rows, cols, weight)[0]
+
+    def _representatives(self, n, keep_device=False):
+        """rep[i] = position of string i's representative under the configured linkage and group_rep; with
+        keep_device also the int32 device tensor of the device path (None on the host path)."""
+        centroid = self._config.group_rep == GROUP_REP_CENTROID
+        star = self._config.linkage == LINKAGE_STAR
+        if self._matches_device is not None:
+            # on the device (csrc/sg_groups.cu, csrc/sg_star.cu)
+            rep, d_rep = (_device.group_star if star else _device.group_reps)(self._matches_device, n, centroid,
+                                                                               keep_device=True)
+        else:
+            # the list was edited by add_match / remove_match: host statement of the same rule
+            rep, d_rep = (self._host_star_reps if star else self._host_group_reps)(n, centroid), None
+        return (rep, d_rep) if keep_device else rep
 
     def _get_indices_of(self, master_side: str, dupe_side: str) -> Tuple[pd.Series, pd.Series]:
         master_strings = self._master
@@ -701,6 +729,9 @@ class StringGrouper(object):
         options = (GROUP_REP_FIRST, GROUP_REP_CENTROID)
         if self._config.group_rep not in options:
             raise Exception(f"Invalid option value for group_rep. The only permitted values are\n {options}")
+        options = (LINKAGE_SINGLE, LINKAGE_STAR)
+        if self._config.linkage not in options:
+            raise Exception(f"Invalid option value for linkage. The only permitted values are\n {options}")
 
     def _validate_tfidf_matrix_dtype(self):
         options = (np.float32, np.float64)
@@ -740,6 +771,48 @@ class StringGrouper(object):
             raise Exception('Both master and master_id must be pandas.Series of the same length.')
         if duplicates is not None and duplicates_id is not None and len(duplicates) != len(duplicates_id):
             raise Exception('Both duplicates and duplicates_id must be pandas.Series of the same length.')
+
+
+def _centroid_weight(graph, pairs):
+    """Similarity sum of every row: `graph` is the CSR pattern of the pairs as _host_group_reps builds it (ref:875-881),
+    summed in storage order within each row like cc_rowsum_kernel."""
+    graph.data = pairs['similarity'].to_numpy()
+    return np.asarray(graph.sum(axis=1)).squeeze(axis=1)
+
+
+def star_representatives(n, rows, cols, weight=None):
+    """(rep, rounds): the star groups of csrc/sg_star.cu in numpy, the same rounds with the same result.
+
+    Strings are ranked by index (weight None) or by weight descending, then index.  Serial rule: in rank order, a
+    string not yet assigned becomes a pivot and takes every unassigned neighbour (u ~ v when the pair (u, v) or (v, u)
+    is listed).  A round decides every undecided v whose undecided neighbours all rank above min(pv, rank[v]), where
+    pv is the smallest rank among v's pivot neighbours; such a v joins the pivot of rank pv, or becomes a pivot when
+    pv > rank[v].  The undecided string of smallest rank is always decided, so the loop ends."""
+    idx = np.arange(n, dtype=np.int64)
+    order = idx if weight is None else np.lexsort((idx, -np.asarray(weight)))
+    rank = np.empty(n, dtype=np.int64)
+    rank[order] = idx
+    rows, cols = np.asarray(rows, dtype=np.int64), np.asarray(cols, dtype=np.int64)
+    off = rows != cols
+    u, v = np.concatenate([rows[off], cols[off]]), np.concatenate([cols[off], rows[off]])
+    none = np.iinfo(np.int64).max
+    rep = np.full(n, -1, dtype=np.int64)
+    pv = np.full(n, none, dtype=np.int64)
+    rounds = 0
+    while (undecided := rep < 0).any():
+        rounds += 1
+        keep = undecided[u]                    # arcs out of decided strings change nothing any more
+        u, v = u[keep], v[keep]
+        to_pivot = rep[v] == v
+        np.minimum.at(pv, u[to_pivot], rank[v[to_pivot]])
+        blk = np.full(n, none, dtype=np.int64)
+        to_open = rep[v] < 0
+        np.minimum.at(blk, u[to_open], rank[v[to_open]])
+        ready = np.nonzero(undecided & (blk > np.minimum(pv, rank)))[0]
+        joins = pv[ready] < rank[ready]
+        rep[ready] = ready
+        rep[ready[joins]] = order[pv[ready[joins]]]
+    return rep, rounds
 
 
 def block_ids_of(master, duplicates=None, master_keys=None, duplicates_keys=None):
