@@ -207,7 +207,10 @@ size_t sg_postings_workspace_bytes(int64_t nnz, int64_t n_cols, int64_t n_tiles)
 int sg_postings_build(int64_t n_rows, int64_t n_cols, int64_t nnz, const int64_t *indptr /*[dev]*/,
                       const int32_t *indices /*[dev]*/, const float *val32 /*[dev]*/,
                       const int32_t *perm /*[dev] or NULL*/, int tile_w, int64_t indptr_base,
-                      float w_scale /* weights are multiplied by this before the fp16 rounding: 1 / max|w| */,
+                      float w_scale /* weights are multiplied by this before the fp16 rounding (1 / largest row
+                                       norm from 1 up, below it the largest power of two at most that, so that every
+                                       weight lies in [-1, 1]); a nonzero weight that rounds to zero keeps the smallest
+                                       fp16 subnormal instead */,
                       void *bucket_dir /*[dev] T*(n_cols+1)*8 B*/, void *bucket_maxw /*[dev] (n_cols+1)*Tp*2 B*/,
                       void *postings /*[dev] nnz*4 B*/, int32_t *n_spilled /*[dev] or NULL*/,
                       void *ws /*[dev]*/, size_t ws_bytes, void *stream);
@@ -280,7 +283,9 @@ int sg_tile_bounds(int64_t n_right, const int32_t *perm /*[dev] position -> row,
  * `group_items` [dev] sg_num_tiles()/tiles_per_group + 1 entries (rounded up) is scratch for the work items of the
  * triangle, required with diag_rank.
  * Block-max test: a (row, column tile) pair is walked only if sum_f |a_f| * max|w_(f,t)| over ALL the row's kept
- * features (bucket_maxw, fp16, rounded up) can reach the pair's threshold.
+ * features (bucket_maxw, fp16, rounded up) can reach the pair's threshold.  The bound and the thresholds it is
+ * tested against are both multiplied by `b_scale` (a power of two in (0, 1]: 1 / a power of two at or above
+ * left norm * right norm, 1 for rows of norm <= 1), so that the bound's fp16 arithmetic works on values below 2.
  */
 #define SG_ACC_F32 0
 #define SG_ACC_U16 1 /* 1/32768 fixed point: caller adds 2e-5 per kept feature to the margin; weights >= 0, scores < 2 */
@@ -294,6 +299,7 @@ int sg_cossim_candidates(const int64_t *a_indptr /*[dev]*/, const int32_t *a_len
                          const int32_t *perm_b /*[dev] position -> right row id, or NULL*/, int tile_w,
                          int acc_dtype,
                          float a_scale /* left weights are multiplied by this: the inverse of w_scale */,
+                         float b_scale /* units of the block-max bound, see above */,
                          float cand_threshold, const float *cand_threshold_row /*[dev] per row id, or NULL*/,
                          const float *pruned_norm_row /*[dev] per row id, or NULL*/,
                          const float *tile_bound /*[dev] sg_num_tiles_padded() entries, zero padded*/,
@@ -329,7 +335,8 @@ int sg_cossim_candidates_floor(const int64_t *a_indptr /*[dev]*/, const int32_t 
                                int64_t n_right, int64_t n_cols, const void *bucket_dir /*[dev]*/,
                                const void *bucket_maxw /*[dev]*/, const void *postings /*[dev]*/,
                                const int32_t *perm_b /*[dev] or NULL*/, int tile_w, int acc_dtype, float a_scale,
-                               float cand_threshold, const float *cand_threshold_row /*[dev] per row id, or NULL*/,
+                               float b_scale, float cand_threshold,
+                               const float *cand_threshold_row /*[dev] per row id, or NULL*/,
                                const float *pruned_norm_row /*[dev] per row id, or NULL*/,
                                const float *tile_bound /*[dev]*/, int64_t tiles_per_group,
                                int32_t *cand_row /*[dev] cap*/, int32_t *cand_col /*[dev] cap*/,
@@ -353,7 +360,8 @@ int sg_cossim_candidates_range(const int64_t *a_indptr /*[dev]*/, const int32_t 
                                int64_t n_right, int64_t n_cols, const void *bucket_dir /*[dev]*/,
                                const void *bucket_maxw /*[dev]*/, const void *postings /*[dev]*/,
                                const int32_t *perm_b /*[dev] or NULL*/, int tile_w, int acc_dtype, float a_scale,
-                               float cand_threshold, const float *cand_threshold_row /*[dev] per row id, or NULL*/,
+                               float b_scale, float cand_threshold,
+                               const float *cand_threshold_row /*[dev] per row id, or NULL*/,
                                const float *pruned_norm_row /*[dev] per row id, or NULL*/,
                                const float *tile_bound /*[dev]*/, int64_t tiles_per_group,
                                const int32_t *lo_pos /*[dev] per left row id*/,

@@ -4,6 +4,7 @@ PyTorch is used for device memory, streams and (in _dist.py) torch.distributed
 only; every kernel on the hot path lives in csrc/*.cu behind the C ABI.
 """
 import ctypes
+import math
 import os
 
 import numpy as np
@@ -40,9 +41,11 @@ CAND_CHUNK = int(os.environ.get("SG_B200_CAND_CHUNK", str(1 << 28)))            
 OPTIMISTIC_PAIRS = float(os.environ.get("SG_B200_OPTIMISTIC_PAIRS", "5e11"))
 REFINE = os.environ.get("SG_B200_REFINE", "1") != "0"      # grouped per-candidate bound before the exact re-score
 # K2 formulation: "row" (the default) = one warp per left row over L2-resident posting buckets (csrc/sg_cossim.cu; also
-# the general path: negative values, norms above 1, near-zero thresholds); "tiles" = right tiles staged through TMA into
-# shared memory (csrc/sg_tiles.cu), for L2-normalised non-negative operands.  Measured on H100 at 663k rows the row kernel
-# is the faster one (65 vs 80 ms per step, DESIGN.md §4).
+# the general path: negative values, row norms other than 1, near-zero thresholds; see candidate_scales); "tiles" =
+# right tiles staged through TMA into shared memory (csrc/sg_tiles.cu), for non-negative operands whose rows have norm
+# <= 1 on both sides.  Measured on H100 at 663k rows the row kernel is the faster one (65 vs 80 ms per step, DESIGN.md
+# §4).  Signed operands need a threshold of at least the candidate margin (cossim_topn); stored values must be finite
+# with nonzero magnitudes in [VALUE_MIN, VALUE_MAX] (DeviceCSR.from_scipy).
 K2_KERNEL = os.environ.get("SG_B200_KERNEL", "row").lower()
 TILE_MARGIN = 2e-5               # fp32 arithmetic of thresholds / norms and the f64 -> f32 copy of the values
 TILE_MARGIN_PER_FEATURE = 3.1e-5  # a_q * w_q / 2^30 vs a * w: both weights rounded to nearest 2^-15 (<= 2^-15 + 2^-32)
@@ -56,6 +59,30 @@ FLOOR_MIN_ROWS = 65536
 DEDUP_MIN_ROWS = 131072
 DEDUP_MIN_SHARE = 0.02
 DEDUP_HASH_MASK = (1 << 64) - 1       # row hash bits the grouping sorts by (tests narrow it to force collisions)
+# magnitudes of nonzero stored values an uploaded matrix may hold: the candidate stage works on an fp32 copy, where
+# every product of two of them and every score stays a positive normal number below fp32's range
+VALUE_MIN, VALUE_MAX = 2.0 ** -50, 2.0 ** 50
+
+
+def candidate_scales(norm_a, norm_b):
+    """(w_scale, a_scale, b_scale) of the row kernel's candidate stage for left rows of norm <= norm_a and right rows
+    of norm <= norm_b.  Right weights are multiplied by w_scale before their fp16 rounding: 1 / norm_b from norm 1 up,
+    below it the largest power of two at most 1 / norm_b, so they lie in [-1, 1] and keep fp16's relative precision
+    however small the right side's values are.  Left weights are multiplied by a_scale = 1 / w_scale, so partial
+    scores stay in score units.  The block-max bound and the thresholds it is tested against are multiplied by
+    b_scale, 1 / a power of two at or above norm_a * norm_b (1 while that is at most 1): the bound's fp16 arithmetic
+    then works on values below 2, where its slack holds (csrc/sg_cossim.cu).  All three are 1 for L2-normalised
+    rows."""
+    w_scale = 1.0 / norm_b if norm_b >= 1.0 else 2.0 ** math.floor(-math.log2(norm_b))
+    scale = norm_a * norm_b
+    b_scale = 1.0 if scale <= 1.0 + 1e-6 else 2.0 ** -math.ceil(math.log2(scale))
+    return w_scale, 1.0 / w_scale, b_scale
+
+
+def fixed_point_ok(A, B):
+    """The 16-bit fixed-point accumulator and the tile kernel take products of weights in [0, 1] (its margins are
+    stated for them) and scores below 2: non-negative operands whose rows have norm <= 1 on both sides."""
+    return A.nonneg and B.nonneg and A.norm_bound <= 1.0 + 1e-6 and B.norm_bound <= 1.0 + 1e-6
 
 
 def torch():
@@ -173,8 +200,21 @@ class DeviceCSR:
         if not issparse(m):
             raise TypeError("expected a scipy sparse matrix, got %r" % type(m))
         m = m.tocsr()
-        if not m.has_sorted_indices:
-            m = m.sorted_indices()
+        # canonical form, as scipy's product sees it: duplicate entries summed, indices sorted, no stored zeros (the
+        # caller's matrix is not modified)
+        if not m.has_canonical_format:
+            m = m.copy()
+            m.sum_duplicates()
+        if m.nnz and not np.all(m.data):
+            m = m.copy()
+            m.eliminate_zeros()
+        if m.nnz:
+            mag = np.abs(m.data)
+            if not np.all(np.isfinite(mag)):
+                raise ValueError("the matrix holds NaN or infinite values")
+            if mag.min() < VALUE_MIN or mag.max() > VALUE_MAX:
+                raise ValueError("stored values must have magnitudes between 2^-50 and 2^50 (found %g .. %g): the "
+                                 "candidate stage multiplies them in fp32" % (mag.min(), mag.max()))
         if m.nnz >= 2**31 - 1:
             raise OverflowError("matrix has %d stored values; int32 indices overflow" % m.nnz)
         dtype = np.float32 if m.dtype == np.float32 else np.float64
@@ -377,8 +417,9 @@ def _build_postings(B, perm, tile_w, n_spilled=None):
     post = _empty(max(B.nnz, 1), t.int32, B.device)
     ws_bytes = int(L.sg_postings_workspace_bytes(B.nnz, n_cols, T))
     ws = _empty(ws_bytes, t.uint8, B.device)
+    w_scale = candidate_scales(1.0, B.norm_bound)[0]
     _lib.check(L.sg_postings_build(n_rows, n_cols, B.nnz, _ptr(B.d_indptr), _ptr(B.d_indices), _ptr(B.d_val32),
-                                   _ptr(perm), tile_w, B.base, 1.0 / max(B.norm_bound, 1.0),
+                                   _ptr(perm), tile_w, B.base, w_scale,
                                    _ptr(bucket_dir), _ptr(bucket_maxw), _ptr(post), _ptr(n_spilled),
                                    _ptr(ws), ws_bytes, _stream()))
     # tile counts, their scan, the per-tile sort, the segmented sort of the spilled tiles and their directory
@@ -692,6 +733,13 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
     if n_rows == 0 or n_right == 0 or top_n <= 0 or A.nnz == 0 or B.nnz == 0:
         z32 = _empty(1, t.int32, dev)
         return DeviceMatches(shape, z32, z32, _empty(1, t.float64, dev), 0, 0)
+    # Candidates are the pairs whose approximate partial score exceeds threshold - margin, clamped at 0.  With signed
+    # weights a positive exact score can cancel to a partial of 0 or less, so the clamp would lose pairs.
+    signed_margin = CAND_MARGIN * max(A.norm_bound * B.norm_bound, 1.0)
+    if not (A.nonneg and B.nonneg) and not float(threshold) >= signed_margin:
+        raise ValueError("operands with negative values need a threshold of at least %.9g (the candidate margin %g "
+                         "times the larger of 1 and the product of the largest row norms), got %r"
+                         % (signed_margin, CAND_MARGIN, threshold))
     if stats is not None:
         stats["blocks"] = blocked
 
@@ -738,7 +786,7 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
     acc = (acc or ACC_DTYPE).lower()
     if acc not in ("u16", "f32"):
         raise ValueError("accumulator dtype must be 'u16' or 'f32', got %r" % (acc,))
-    if not (A.nonneg and B.nonneg and scale <= 1.0 + 1e-6) or thr_c < 0.05:
+    if not fixed_point_ok(A, B) or thr_c < 0.05:
         acc = "f32"      # also near-zero thresholds: a tiny positive score must not round to a fixed-point zero
     acc_code = _lib.SG_ACC_U16 if acc == "u16" else _lib.SG_ACC_F32
     margin_pf = U16_MARGIN_PER_FEATURE if acc == "u16" else 0.0
@@ -760,6 +808,7 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
     if use_tiles:
         margin = TILE_MARGIN * max(scale, 1.0)
         margin_pf = TILE_MARGIN_PER_FEATURE
+    _, a_scale, b_scale = candidate_scales(A.norm_bound, B.norm_bound)
     prune_auto = prune is None          # the caller left the level open: it may be lowered, see below
     prune = PRUNE_FRAC if prune is None else float(prune)
     counters = t.zeros(4, dtype=t.int64, device=dev)       # [0] cand_count, [1] work queue
@@ -854,7 +903,7 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
             _lib.check(L.sg_cossim_candidates_range(
                 _ptr(A.d_indptr), _ptr(l_len), _ptr(l_idx), _ptr(l_val), rb, re_, _ptr(perm), n_right, A.shape[1],
                 _ptr(bucket_dir), _ptr(bucket_maxw), _ptr(post), _ptr(perm_b), tile_w, acc_code,
-                max(B.norm_bound, 1.0), thr_c, _ptr(l_thr), _ptr(l_xp), _ptr(tile_bound), tiles_per_group,
+                a_scale, b_scale, thr_c, _ptr(l_thr), _ptr(l_xp), _ptr(tile_bound), tiles_per_group,
                 _ptr(diag_rank), _ptr(hi_pos), _ptr(group_items), _ptr(row_buf), _ptr(col_buf), _ptr(partial_buf),
                 capacity, c_count, c_queue, warps, _stream()))
             LAUNCH_COUNTS["candidates"] += 1
@@ -862,9 +911,9 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
         _lib.check(L.sg_cossim_candidates(
             _ptr(A.d_indptr), _ptr(l_len), _ptr(l_idx), _ptr(l_val), rb, re_, _ptr(perm), n_right,
             A.shape[1], _ptr(bucket_dir), _ptr(bucket_maxw), _ptr(post), _ptr(perm_b), tile_w, acc_code,
-            max(B.norm_bound, 1.0),
-            thr_c, _ptr(l_thr), _ptr(l_xp), _ptr(tile_bound), tiles_per_group, _ptr(diag_rank), _ptr(group_items),
-            _ptr(row_buf), _ptr(col_buf), _ptr(partial_buf), capacity, c_count, c_queue, warps, _stream()))
+            a_scale, b_scale, thr_c, _ptr(l_thr), _ptr(l_xp), _ptr(tile_bound), tiles_per_group, _ptr(diag_rank),
+            _ptr(group_items), _ptr(row_buf), _ptr(col_buf), _ptr(partial_buf), capacity, c_count, c_queue, warps,
+            _stream()))
         LAUNCH_COUNTS["candidates"] += 1
 
     # Exact threshold pruning of the left rows (the fixed-point tile always takes per-row thresholds: its margin
@@ -1201,8 +1250,9 @@ def _cossim_topn_floor(A, B, top_n, threshold, row_begin, row_end, tile_w, stats
     acc = (acc or ACC_DTYPE).lower()
     if acc not in ("u16", "f32"):
         raise ValueError("accumulator dtype must be 'u16' or 'f32', got %r" % (acc,))
-    if scale > 1.0 + 1e-6 or thr_c < 0.05:
+    if not fixed_point_ok(A, B) or thr_c < 0.05:
         acc = "f32"
+    _, a_scale, b_scale = candidate_scales(A.norm_bound, B.norm_bound)
     acc_code = _lib.SG_ACC_U16 if acc == "u16" else _lib.SG_ACC_F32
     margin_pf = U16_MARGIN_PER_FEATURE if acc == "u16" else 0.0
     no_threshold = threshold <= 0.0
@@ -1258,7 +1308,7 @@ def _cossim_topn_floor(A, B, top_n, threshold, row_begin, row_end, tile_w, stats
         _lib.check(L.sg_cossim_candidates(
             _ptr(A.d_indptr), _ptr(l_len), _ptr(l_idx), _ptr(l_val), row_begin, row_begin + int(sample.numel()),
             _ptr(sample), n_right, A.shape[1], _ptr(bucket_dir), _ptr(bucket_maxw), _ptr(post), _ptr(perm_b), tile_w,
-            acc_code, max(B.norm_bound, 1.0), thr_c, _ptr(l_thr), _ptr(l_xp), _ptr(tile_bound), tiles_per_group,
+            acc_code, a_scale, b_scale, thr_c, _ptr(l_thr), _ptr(l_xp), _ptr(tile_bound), tiles_per_group,
             None, None, _ptr(dummy), _ptr(dummy), None, 0, c_count, c_queue, warps, _stream()))
         LAUNCH_COUNTS["candidates"] += 1
         est_usual = int(counters[0].item()) * stride
@@ -1282,7 +1332,7 @@ def _cossim_topn_floor(A, B, top_n, threshold, row_begin, row_end, tile_w, stats
         _lib.check(L.sg_cossim_candidates_floor(
             _ptr(A.d_indptr), _ptr(l_len), _ptr(l_idx), _ptr(l_val), row_begin, row_begin + n, _ptr(perm), n_right,
             A.shape[1], _ptr(bucket_dir), _ptr(bucket_maxw), _ptr(post), _ptr(perm_b), tile_w, acc_code,
-            max(B.norm_bound, 1.0), thr_c, _ptr(l_thr), _ptr(l_xp), _ptr(tile_bound), tiles_per_group, _ptr(row_buf),
+            a_scale, b_scale, thr_c, _ptr(l_thr), _ptr(l_xp), _ptr(tile_bound), tiles_per_group, _ptr(row_buf),
             _ptr(col_buf), _ptr(part_buf), capacity, c_count, c_queue, warps, _ptr(floor_buf), top_n, margin,
             margin_pf, _ptr(self_rank), _lib.SG_FLOOR_SEED if seed else 0, _stream()))
         LAUNCH_COUNTS["candidates"] += 1

@@ -69,12 +69,12 @@ SIGNATURES = {
     "sg_heavy_norms": (_i32, [_i64, _i64, _p, _p, _p, _p, _p, _p, _p]),
     "sg_tile_bounds": (_i32, [_i64, _p, _p, _i32, _p, _p]),
     "sg_cossim_candidates": (_i32, [_p, _p, _p, _p, _i64, _i64, _p, _i64, _i64, _p, _p, _p, _p, _i32, _i32, _f32,
-                                    _f32, _p, _p, _p, _i64, _p, _p, _p, _p, _p, _i64, _p, _p, _i32, _p]),
+                                    _f32, _f32, _p, _p, _p, _i64, _p, _p, _p, _p, _p, _i64, _p, _p, _i32, _p]),
     "sg_cossim_candidates_floor": (_i32, [_p, _p, _p, _p, _i64, _i64, _p, _i64, _i64, _p, _p, _p, _p, _i32, _i32,
-                                          _f32, _f32, _p, _p, _p, _i64, _p, _p, _p, _i64, _p, _p, _i32, _p, _i32,
+                                          _f32, _f32, _f32, _p, _p, _p, _i64, _p, _p, _p, _i64, _p, _p, _i32, _p, _i32,
                                           _f32, _f32, _p, _i32, _p]),
     "sg_cossim_candidates_range": (_i32, [_p, _p, _p, _p, _i64, _i64, _p, _i64, _i64, _p, _p, _p, _p, _i32, _i32,
-                                          _f32, _f32, _p, _p, _p, _i64, _p, _p, _p, _p, _p, _p, _i64, _p, _p, _i32,
+                                          _f32, _f32, _f32, _p, _p, _p, _i64, _p, _p, _p, _p, _p, _p, _i64, _p, _p, _i32,
                                           _p]),
     "sg_tiles_tile_w": (_i32, []),
     "sg_tiles_max_cols": (_i64, []),

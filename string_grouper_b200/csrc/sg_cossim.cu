@@ -32,14 +32,18 @@ namespace sg {
 // candidate scores only have to be within CAND_MARGIN of the exact ones (every candidate is re-scored in the
 // matrix dtype): an fp16 weight is off by at most 2^-11 relative, so a score by at most 4.9e-4.  The order inside a
 // bucket is arbitrary (a bucket holds every column once; the fixed-point tiles add integers, so the candidate set
-// does not depend on it).
+// does not depend on it).  A nonzero weight below fp16's range keeps its sign and becomes the smallest subnormal
+// (2^-24) instead of zero, which is no further from it than rounding to nearest: with the candidate threshold at 0
+// (thresholds below the margin) a pair of non-negative rows is found exactly when it shares a feature.
 constexpr int PB_THREADS = 1024;
 constexpr int PB_ITEMS = 8;
 constexpr int PB_CAP = PB_THREADS * PB_ITEMS;   // postings of a tile sorted in shared memory; larger tiles: global
 constexpr size_t PB_SMEM = (size_t)PB_CAP * 8;  // keys + postings (the block sort's scratch reuses them)
 
 __device__ __forceinline__ uint32_t make_posting(float v, float w_scale, uint32_t local) {
-    return ((uint32_t)__half_as_ushort(__float2half_rn(v * w_scale)) << 16) | local;
+    const float x = v * w_scale;
+    const float y = x != 0.f && fabsf(x) < 0x1p-24f ? copysignf(0x1p-24f, x) : x;
+    return ((uint32_t)__half_as_ushort(__float2half_rn(y)) << 16) | local;
 }
 
 // postings per tile, one warp per tile; tile_cnt[T] = 0 closes the exclusive scan into tile_off
@@ -394,6 +398,10 @@ __device__ __forceinline__ void apply_buckets(AccT *__restrict__ acc, const uint
 // once per 64-tile batch, with the same fp16 round-up and a slack of 5e-4 per feature.  Every hfma2
 // rounds once; while the running sum stays below 2 (ulp 2^-10) that is at most 2^-11 < 5e-4, and once it reaches 2
 // it stays there (non-negative terms, monotone rounding), above any threshold of scores in [0, 1].
+// `b_scale` (a power of two, 1 for rows of norm <= 1) keeps that argument for any operands: the left weights of the
+// bound and the thresholds it is tested against are multiplied by it, so the bound is evaluated in units of a power
+// of two at or above the largest possible score, where every term and every threshold lies below 2 (and nothing
+// overflows fp16).  The accumulated partial scores stay in score units.
 struct FloorArgs {
     float *floor;
     const int32_t *self_rank;
@@ -427,7 +435,7 @@ candidates_body(const int64_t *__restrict__ a_indptr, const int32_t *__restrict_
                 int64_t row_end, const int32_t *__restrict__ perm_a, int64_t n_right,
                 const int2 *__restrict__ bdir, const uint32_t *__restrict__ maxw_h,
                 const uint32_t *__restrict__ post, const int32_t *__restrict__ perm_b, int Tp, int W,
-                int64_t T, int64_t tiles_per_group, float a_scale, float thr_all,
+                int64_t T, int64_t tiles_per_group, float a_scale, float b_scale, float thr_all,
                 const float *__restrict__ thr_row, const float *__restrict__ xp_norm,
                 const float *__restrict__ tile_bound, const int32_t *__restrict__ diag_rank,
                 const unsigned long long *__restrict__ group_items, int32_t *__restrict__ cand_row,
@@ -517,7 +525,7 @@ candidates_body(const int64_t *__restrict__ a_indptr, const int32_t *__restrict_
             f0 = a_idx[p0 + lane];
             const float a = a_val[p0 + lane] * a_scale;
             a0 = Ops::left_weight(a);
-            a2 = __half2half2(__float2half_ru(fabsf(a)));   // rounded up: the bound must not fall short
+            a2 = __half2half2(__float2half_ru(fabsf(a * b_scale)));   // rounded up: the bound must not fall short
         }
         const int2 *drow = bdir + f0 * n_tiles;
         const int nk = nf < 32 ? nf : 32;
@@ -563,7 +571,7 @@ candidates_body(const int64_t *__restrict__ a_indptr, const int32_t *__restrict_
                     __half2 al = __float2half2_rn(0.f);
                     if (base + lane < nf) {
                         fl = a_idx[p0 + base + lane];
-                        al = __half2half2(__float2half_ru(fabsf(a_val[p0 + base + lane] * a_scale)));
+                        al = __half2half2(__float2half_ru(fabsf(a_val[p0 + base + lane] * a_scale * b_scale)));
                     }
                     const int nc = nf - base < 32 ? nf - base : 32;
                     for (int kk = 0; kk < nc; ++kk) {
@@ -577,8 +585,8 @@ candidates_body(const int64_t *__restrict__ a_indptr, const int32_t *__restrict_
                 const float2 tb2 = reinterpret_cast<const float2 *>(tile_bound)[(tb >> 1) + lane];
                 const float thr0 = xp > 0.f ? fmaxf(fmaf(-xp, tb2.x, thr_r), 0.f) : thr_r;
                 const float thr1 = xp > 0.f ? fmaxf(fmaf(-xp, tb2.y, thr_r), 0.f) : thr_r;
-                m_even = __ballot_sync(FULL, t0 < t_end && up0 && ub.x + slack > thr0);
-                m_odd = __ballot_sync(FULL, t0 + 1 < t_end && up1 && ub.y + slack > thr1);
+                m_even = __ballot_sync(FULL, t0 < t_end && up0 && ub.x + slack > thr0 * b_scale);
+                m_odd = __ballot_sync(FULL, t0 + 1 < t_end && up1 && ub.y + slack > thr1 * b_scale);
             }
             // ---- walk the surviving tiles; the directory entry of the next one is fetched ahead
             int t = -1;
@@ -687,7 +695,7 @@ candidates_body(const int64_t *__restrict__ a_indptr, const int32_t *__restrict_
         const float *__restrict__ a_val, int64_t row_begin, int64_t row_end, const int32_t *__restrict__ perm_a,    \
         int64_t n_right, const int2 *__restrict__ bdir, const uint32_t *__restrict__ maxw_h,                        \
         const uint32_t *__restrict__ post, const int32_t *__restrict__ perm_b, int Tp, int W, int64_t T,            \
-        int64_t tiles_per_group, float a_scale, float thr_all, const float *__restrict__ thr_row,                   \
+        int64_t tiles_per_group, float a_scale, float b_scale, float thr_all, const float *__restrict__ thr_row,    \
         const float *__restrict__ xp_norm, const float *__restrict__ tile_bound,                                    \
         const int32_t *__restrict__ diag_rank, const unsigned long long *__restrict__ group_items,                  \
         int32_t *__restrict__ cand_row, int32_t *__restrict__ cand_col, float *__restrict__ cand_partial,           \
@@ -695,7 +703,7 @@ candidates_body(const int64_t *__restrict__ a_indptr, const int32_t *__restrict_
         unsigned long long *__restrict__ row_queue
 #define SG_CAND_ARGS                                                                                              \
     a_indptr, a_len, a_idx, a_val, row_begin, row_end, perm_a, n_right, bdir, maxw_h, post, perm_b, Tp, W, T,     \
-        tiles_per_group, a_scale, thr_all, thr_row, xp_norm, tile_bound, diag_rank, group_items, cand_row,        \
+        tiles_per_group, a_scale, b_scale, thr_all, thr_row, xp_norm, tile_bound, diag_rank, group_items, cand_row, \
         cand_col, cand_partial, cap, cand_count, row_queue
 
 template <int NW, typename AccT>
@@ -1403,7 +1411,7 @@ static int launch_candidates(const int64_t *a_indptr, const int32_t *a_len, cons
                              const float *a_val32, int64_t row_begin, int64_t row_end, const int32_t *perm_a,
                              int64_t n_right, int64_t n_cols, const void *bucket_dir, const void *bucket_maxw,
                              const void *postings, const int32_t *perm_b, int tile_w, int64_t tiles_per_group,
-                             float a_scale,
+                             float a_scale, float b_scale,
                              float thr_c, const float *thr_row, const float *xp_norm, const float *tile_bound,
                              const int32_t *diag_rank, unsigned long long *group_items,
                              int32_t *cand_row, int32_t *cand_col, float *cand_partial,
@@ -1444,7 +1452,7 @@ static int launch_candidates(const int64_t *a_indptr, const int32_t *a_len, cons
 #define SG_KARGS                                                                                                    \
     a_indptr, a_len, a_indices, a_val32, row_begin, row_end, perm_a, n_right, (const int2 *)bucket_dir,               \
         (const uint32_t *)bucket_maxw, (const uint32_t *)postings, perm_b, (int)sg_num_tiles_padded(n_right, tile_w), \
-        tile_w, T, tiles_per_group, a_scale, thr_c, thr_row, xp_norm, tile_bound, diag_rank,                         \
+        tile_w, T, tiles_per_group, a_scale, b_scale, thr_c, thr_row, xp_norm, tile_bound, diag_rank,                \
         diag_rank ? group_items : nullptr, cand_row, cand_col, cand_partial, (unsigned long long)cand_cap, cand_count, \
         row_queue
     if constexpr (RANGE)
@@ -1463,7 +1471,7 @@ static int cossim_candidates(const int64_t *a_indptr, const int32_t *a_len, cons
                              const float *a_val32, int64_t row_begin, int64_t row_end, const int32_t *perm_a,
                              int64_t n_right, int64_t n_cols, const void *bucket_dir, const void *bucket_maxw,
                              const void *postings, const int32_t *perm_b, int tile_w, int acc_dtype, float a_scale,
-                             float cand_threshold,
+                             float b_scale, float cand_threshold,
                              const float *cand_threshold_row, const float *pruned_norm_row, const float *tile_bound,
                              int64_t tiles_per_group, const int32_t *diag_rank, unsigned long long *group_items,
                              int32_t *cand_row, int32_t *cand_col, float *cand_partial, int64_t cand_cap,
@@ -1482,6 +1490,7 @@ static int cossim_candidates(const int64_t *a_indptr, const int32_t *a_len, cons
         return fail(SG_ERR_INVALID, "tile_w must be a multiple of 32 and tile_w * accumulator size a multiple of 256 bytes");
     if (tile_w > 32768) return fail(SG_ERR_INVALID, "tile_w must not exceed 32768 (16-bit bucket lengths)");
     if (!(cand_threshold >= 0.f)) return fail(SG_ERR_INVALID, "cand_threshold must be >= 0");
+    if (!(b_scale > 0.f && b_scale <= 1.f)) return fail(SG_ERR_INVALID, "b_scale must be in (0, 1]");
     int dev = 0, n_sm = 0, smem_optin = 0;
     SG_CUDA_TRY(cudaGetDevice(&dev));
     SG_CUDA_TRY(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev));
@@ -1491,8 +1500,9 @@ static int cossim_candidates(const int64_t *a_indptr, const int32_t *a_len, cons
                     (size_t)warps_per_cta * tile_w * acc_bytes, smem_optin);
 #define SG_ARGS                                                                                              \
     a_indptr, a_len, a_indices, a_val32, row_begin, row_end, perm_a, n_right, n_cols, bucket_dir, bucket_maxw, \
-        postings, perm_b, tile_w, tiles_per_group, a_scale, cand_threshold, cand_threshold_row, pruned_norm_row,      \
-        tile_bound, diag_rank, group_items, cand_row, cand_col, cand_partial, cand_cap, cand_count, row_queue, n_sm, st
+        postings, perm_b, tile_w, tiles_per_group, a_scale, b_scale, cand_threshold, cand_threshold_row,           \
+        pruned_norm_row, tile_bound, diag_rank, group_items, cand_row, cand_col, cand_partial, cand_cap, cand_count, \
+        row_queue, n_sm, st
     if (hi_pos) {
         // the range variant is built for the default 8 warps only
         if (warps_per_cta != 8) return fail(SG_ERR_INVALID, "the position-range variant runs with 8 warps per CTA");
@@ -1529,15 +1539,16 @@ int sg_cossim_candidates(const int64_t *a_indptr, const int32_t *a_len, const in
                          const float *a_val32, int64_t row_begin, int64_t row_end, const int32_t *perm_a,
                          int64_t n_right, int64_t n_cols, const void *bucket_dir, const void *bucket_maxw,
                          const void *postings, const int32_t *perm_b, int tile_w, int acc_dtype, float a_scale,
-                         float cand_threshold,
+                         float b_scale, float cand_threshold,
                          const float *cand_threshold_row, const float *pruned_norm_row, const float *tile_bound,
                          int64_t tiles_per_group, const int32_t *diag_rank, unsigned long long *group_items,
                          int32_t *cand_row, int32_t *cand_col, float *cand_partial, int64_t cand_cap,
                          unsigned long long *cand_count, unsigned long long *row_queue, int warps_per_cta,
                          void *stream_) {
     return cossim_candidates(a_indptr, a_len, a_indices, a_val32, row_begin, row_end, perm_a, n_right, n_cols,
-                             bucket_dir, bucket_maxw, postings, perm_b, tile_w, acc_dtype, a_scale, cand_threshold,
-                             cand_threshold_row, pruned_norm_row, tile_bound, tiles_per_group, diag_rank, group_items,
+                             bucket_dir, bucket_maxw, postings, perm_b, tile_w, acc_dtype, a_scale, b_scale,
+                             cand_threshold, cand_threshold_row, pruned_norm_row, tile_bound, tiles_per_group,
+                             diag_rank, group_items,
                              cand_row, cand_col, cand_partial, cand_cap, cand_count, row_queue, warps_per_cta, stream_,
                              nullptr);
 }
@@ -1546,7 +1557,8 @@ int sg_cossim_candidates_floor(const int64_t *a_indptr, const int32_t *a_len, co
                                const float *a_val32, int64_t row_begin, int64_t row_end, const int32_t *perm_a,
                                int64_t n_right, int64_t n_cols, const void *bucket_dir, const void *bucket_maxw,
                                const void *postings, const int32_t *perm_b, int tile_w, int acc_dtype, float a_scale,
-                               float cand_threshold, const float *cand_threshold_row, const float *pruned_norm_row,
+                               float b_scale, float cand_threshold, const float *cand_threshold_row,
+                               const float *pruned_norm_row,
                                const float *tile_bound, int64_t tiles_per_group, int32_t *cand_row,
                                int32_t *cand_col, float *cand_partial, int64_t cand_cap,
                                unsigned long long *cand_count, unsigned long long *row_queue, int warps_per_cta,
@@ -1562,8 +1574,9 @@ int sg_cossim_candidates_floor(const int64_t *a_indptr, const int32_t *a_len, co
     if (self_rank && !perm_a) return fail(SG_ERR_INVALID, "self_rank needs perm_a");
     const FloorArgs fa{row_floor, self_rank, seed ? 1 : 0, top_n, floor_margin, floor_margin_per_feature};
     return cossim_candidates(a_indptr, a_len, a_indices, a_val32, row_begin, row_end, perm_a, n_right, n_cols,
-                             bucket_dir, bucket_maxw, postings, perm_b, tile_w, acc_dtype, a_scale, cand_threshold,
-                             cand_threshold_row, pruned_norm_row, tile_bound, tiles_per_group, nullptr, nullptr,
+                             bucket_dir, bucket_maxw, postings, perm_b, tile_w, acc_dtype, a_scale, b_scale,
+                             cand_threshold, cand_threshold_row, pruned_norm_row, tile_bound, tiles_per_group,
+                             nullptr, nullptr,
                              cand_row, cand_col, cand_partial, cand_cap, cand_count, row_queue, warps_per_cta, stream_,
                              &fa);
 }
@@ -1572,7 +1585,8 @@ int sg_cossim_candidates_range(const int64_t *a_indptr, const int32_t *a_len, co
                                const float *a_val32, int64_t row_begin, int64_t row_end, const int32_t *perm_a,
                                int64_t n_right, int64_t n_cols, const void *bucket_dir, const void *bucket_maxw,
                                const void *postings, const int32_t *perm_b, int tile_w, int acc_dtype, float a_scale,
-                               float cand_threshold, const float *cand_threshold_row, const float *pruned_norm_row,
+                               float b_scale, float cand_threshold, const float *cand_threshold_row,
+                               const float *pruned_norm_row,
                                const float *tile_bound, int64_t tiles_per_group, const int32_t *lo_pos,
                                const int32_t *hi_pos, unsigned long long *group_items, int32_t *cand_row,
                                int32_t *cand_col, float *cand_partial, int64_t cand_cap,
@@ -1580,8 +1594,9 @@ int sg_cossim_candidates_range(const int64_t *a_indptr, const int32_t *a_len, co
                                void *stream_) {
     if (!lo_pos || !hi_pos || !group_items) return fail(SG_ERR_INVALID, "lo_pos, hi_pos and group_items are required");
     return cossim_candidates(a_indptr, a_len, a_indices, a_val32, row_begin, row_end, perm_a, n_right, n_cols,
-                             bucket_dir, bucket_maxw, postings, perm_b, tile_w, acc_dtype, a_scale, cand_threshold,
-                             cand_threshold_row, pruned_norm_row, tile_bound, tiles_per_group, lo_pos, group_items,
+                             bucket_dir, bucket_maxw, postings, perm_b, tile_w, acc_dtype, a_scale, b_scale,
+                             cand_threshold, cand_threshold_row, pruned_norm_row, tile_bound, tiles_per_group,
+                             lo_pos, group_items,
                              cand_row, cand_col, cand_partial, cand_cap, cand_count, row_queue, warps_per_cta, stream_,
                              nullptr, hi_pos);
 }

@@ -12,6 +12,11 @@ Semantics (SURVEY.md Appendix A.3 / A.4): per row of A the `top_n` largest entri
 unspecified upstream — the same value-descending rows are returned.  Among EQUAL values at the top-n cut the larger
 column is kept (what the upstream first-touch / reverse-block traversals yield for identical rows).
 `threshold=None` means "no threshold": supported for non-negative operands, where it equals "strictly positive".
+Any float32 / float64 matrix is accepted: it is made canonical first (duplicate entries summed, indices sorted, stored
+zeros dropped, as scipy's own product sees it), and the result is that of the exact product.  Refused up front:
+NaN / infinite values and nonzero magnitudes outside [2^-50, 2^50] (ValueError); operands with negative values with
+`threshold=None` or a negative one (NotImplementedError) or below CAND_MARGIN * max(1, product of the largest row
+norms) (ValueError), where a positive score could cancel in the approximate candidate stage.
 """
 import ctypes
 

@@ -22,7 +22,10 @@ def _expected(m, perm, W, w_scale):
     lens = np.diff(m.indptr)
     p = np.repeat(pos, lens)
     t = p // W
-    w = (m.data.astype(np.float32) * np.float32(w_scale)).astype(np.float16)   # fp32 product, RN to fp16
+    x = m.data.astype(np.float32) * np.float32(w_scale)
+    w = x.astype(np.float16)                                                     # fp32 product, RN to fp16
+    # a nonzero weight that rounds to zero keeps its sign and becomes the smallest subnormal
+    w = np.where((w == 0) & (x != 0), np.copysign(np.float16(2.0 ** -24), x), w).astype(np.float16)
     post = (w.view(np.uint16).astype(np.uint32) << 16) | (p - t * W).astype(np.uint32)
     return m.indices.astype(np.int64) * T + t, post, T
 
@@ -42,7 +45,7 @@ def _check(m, W, perm=None):
     maxw = bmaxw.cpu().numpy().view(np.uint16).reshape(V1, Tp)
     gpost = post.cpu().numpy().view(np.uint32)[:m.nnz]
 
-    b, epost, T_np = _expected(m, perm, W, 1.0 / max(B.norm_bound, 1.0))
+    b, epost, T_np = _expected(m, perm, W, D.candidate_scales(1.0, B.norm_bound)[0])
     assert T == T_np
     elen = np.bincount(b, minlength=V1 * T)
     emax = np.zeros(V1 * T, dtype=np.uint32)
@@ -90,11 +93,13 @@ def test_empty_rows_and_a_feature_in_every_tile(W):
     assert _check(m, W, np.arange(1000, dtype=np.int32)) == 0
 
 
-def test_fp16_subnormal_weights():
+def test_fp16_subnormal_weights_and_weights_below_fp16():
+    """weights in fp16's subnormal range, and below it: those keep their sign as the smallest subnormal (2^-24)"""
     rng = np.random.default_rng(8)
     m = sp.random(700, 200, density=0.05, format="csr", random_state=rng, dtype=np.float64)
     m.data *= 10.0 ** rng.integers(-9, 0, size=m.nnz)           # below 6.1e-5 is subnormal, below 3e-8 zero in fp16
-    assert (np.abs(m.data) < 6.1e-5).sum() > 100
+    m.data[::7] *= -1
+    assert (np.abs(m.data) < 6.1e-5).sum() > 100 and (np.abs(m.data) * 4 < 2.0 ** -25).sum() > 100
     assert _check(m, 128) == 0
 
 
