@@ -6,7 +6,7 @@
 // and the vstack over left blocks (:750).  See DESIGN.md §K2 for the layout.
 //
 //   postings_build   right matrix  -> (feature, column-tile) bucketed postings + directory with block maxima
-//   candidates       block-max test of 64 tiles at a time, then the Gustavson row-wise product of the pruned left
+//   candidates       block-max test of 128 tiles at a time, then the Gustavson row-wise product of the pruned left
 //                    row over the surviving tiles into a shared-memory accumulator tile per warp (16-bit fixed
 //                    point or fp32); emits (row, col) with partial score > the (row, tile) candidate threshold
 //   rescore          exact sorted-merge dot product of every candidate pair; rescore_refined first drops the
@@ -208,10 +208,6 @@ constexpr int LONG_BUCKET = 64;  // buckets from this length on are streamed by 
 #ifndef SG_WALK_MLP
 #define SG_WALK_MLP 1            // steps of the concatenated walk whose posting loads are in flight together
 #endif
-#ifndef SG_FILTER_MLP
-#define SG_FILTER_MLP 1          // block-maxima loads in flight per lane in the block-max test
-// With 40 resident warps the load latency is covered; more loads in flight cost registers and issue slots.
-#endif
 
 // Resident CTAs per SM the register allocation is made for (the accumulator tiles are small, registers decide):
 // 32 warps/CTA x 2 = 64 warps at 32 registers; 16 x 3 = 48 warps at 40; 8 x 5 = 40 warps at 48; 4 x 8 = 32 warps at 64.
@@ -361,10 +357,11 @@ __device__ __forceinline__ void apply_buckets(AccT *__restrict__ acc, const uint
 // = the row's threshold minus what the pruned features can still add for the columns of that tile.
 //
 // Block-max test (`maxw_h`, the fp16 largest |weight| of every (feature, tile) bucket, feature-major, rows padded to
-// Tp tiles): no column of tile t can collect more than ub(t) = sum_f |a_f| * max|w_(f,t)|.  The bounds of 64 tiles
-// are evaluated at once, two tiles per lane in packed fp16 (one HFMA2 per kept feature and tile pair), and only
-// the tiles whose bound can exceed their candidate threshold are walked at all: nothing is accumulated, cleared
-// or swept for the others.
+// Tp tiles): no column of tile t can collect more than ub(t) = sum_f |a_f| * max|w_(f,t)|.  The bounds of 128 tiles
+// are evaluated in one pass, four consecutive tiles per lane: per kept feature one 8-byte load of their maxima and two
+// HFMA2 in packed fp16, at an address that is the feature's row offset (held by its lane for the whole row) plus the
+// pass's column.  Only the tiles whose bound can exceed their candidate threshold are walked at all: nothing is
+// accumulated, cleared or swept for the others.
 //
 // Triangle of a self-match (`diag_rank` != NULL, left and right rows the same matrix in the same processing order):
 // row i only reports columns whose position in that order is >= diag_rank[i], so every unordered pair is found
@@ -383,19 +380,19 @@ __device__ __forceinline__ void apply_buckets(AccT *__restrict__ acc, const uint
 // Top-n floor (cossim_candidates_floor_kernel, top_n <= 32, non-negative weights): floor[row] is a proven lower bound
 // of the exact score of the row's top_n-th best pair; it only rises.  A pair whose exact score is below it cannot be
 // in the row's output, so the candidate threshold of the row becomes max(thr_row, floor - E_r - FLOOR_EPS), read again
-// at every 64-tile batch (block-max ballot and sweep).  E_r = margin + margin_pf * kept features bounds how far the
+// at every 128-tile pass (block-max test and sweep).  E_r = margin + margin_pf * kept features bounds how far the
 // accumulated partial p^ can differ from the kept-feature product x_S.y in EITHER direction (the fp16 posting weights
 // and the fixed-point / fp32 roundings are symmetric; the same constants give thr_row), and x_S.y <= exact for
 // non-negative weights.  So p^ - E_r (rounded down) is a lower bound of the exact score of every reported pair: the
 // warp keeps the best 32 of them per work item, one per lane, and once top_n exist publishes the top_n-th with
 // atomicMax (non-negative floats order like their bits).  The pairs of one item are distinct columns.
 // Self-match (`self_rank` = every row's position in the common processing order): `seed` = 1 walks only the row's own
-// column-tile group, starting at the 64-tile batch that holds the row (clusters of identical names sit next to each
+// column-tile group, starting at the 128-tile pass that holds the row (clusters of identical names sit next to each
 // other in that order, so this is where floors rise first); `seed` = 0 walks every other group.
 //
 // Long rows (more than 32 kept features: long records rows, names without a threshold): only the first 32 stay in
-// registers, but ub(t) is taken over ALL kept features, the later ones 32 at a time, their {feature, weight} loaded
-// once per 64-tile batch, with the same fp16 round-up and a slack of 5e-4 per feature.  Every hfma2
+// registers, but ub(t) is taken over ALL kept features, the later ones 32 at a time, their {row offset, weight} loaded
+// once per 128-tile pass, with the same fp16 round-up and a slack of 5e-4 per feature.  Every hfma2
 // rounds once; while the running sum stays below 2 (ulp 2^-10) that is at most 2^-11 < 5e-4, and once it reaches 2
 // it stays there (non-negative terms, monotone rounding), above any threshold of scores in [0, 1].
 // `b_scale` (a power of two, 1 for rows of norm <= 1) keeps that argument for any operands: the left weights of the
@@ -466,7 +463,7 @@ candidates_body(const int64_t *__restrict__ a_indptr, const int32_t *__restrict_
         if (fa.self_rank) n_items = (unsigned long long)n_rows * (unsigned long long)(fa.seed ? 1 : n_groups - 1);
     }
     const int n_tiles = (int)T;
-    int64_t group = 0;          // with group_items: items arrive in increasing order, so the group only moves forward
+    int group = 0;              // with group_items: items arrive in increasing order, so the group only moves forward
     for (;;) {
         unsigned long long item = 0;
         if (lane == 0) item = atomicAdd(row_queue, 1ull);
@@ -478,18 +475,18 @@ candidates_body(const int64_t *__restrict__ a_indptr, const int32_t *__restrict_
             ridx = (int64_t)(item - group_items[group]);
             if constexpr (RANGE) ridx += (int64_t)group_items[n_groups + 1 + group];
         } else {
-            group = (int64_t)(item / (unsigned long long)n_rows);
+            group = (int)(item / (unsigned long long)n_rows);
             ridx = (int64_t)(item % (unsigned long long)n_rows);
         }
         const int64_t row = perm_a ? perm_a[ridx] : row_begin + ridx;   // processing order: neighbours share buckets
-        int own_batch = 0;      // floor seed: the walk starts at the 64-tile batch holding the row
+        int own_pass = 0;       // floor seed: the walk starts at the 128-tile pass holding the row
         if constexpr (FLOOR) {
             if (fa.self_rank) {
                 const int64_t pos = fa.self_rank[row];
                 const int64_t own = pos / (tiles_per_group * W);
                 if (fa.seed) {
-                    group = own;
-                    own_batch = (int)((pos / W - own * tiles_per_group) >> 6);
+                    group = (int)own;
+                    own_pass = (int)((pos / W - own * tiles_per_group) >> 7);
                 } else if (group >= own) {
                     ++group;
                 }
@@ -514,90 +511,97 @@ candidates_body(const int64_t *__restrict__ a_indptr, const int32_t *__restrict_
             const int t_hi = (int)(((int64_t)hr + W - 1) / W);
             if (t_hi < t_end) t_end = t_hi;
         }
-        const int t_first = (int)(((int64_t)dr / W) & ~63);            // first 64-tile batch at or above the rank
+        const int t_first = (int)(((int64_t)dr / W) & ~127);           // the 128-tile pass holding the rank
         const int tb_begin = t_first > t_begin ? t_first : t_begin;
 
-        // the first 32 features of the row stay in registers
+        // the first 32 features of the row stay in registers; lane k also holds where its feature's block maxima row
+        // starts, in 4-tile (8-byte) units: below T * V1 < 2^31 (checked by sg_postings_build), so 32 bits
         int f0 = 0;
         float a0 = 0.f;
         __half2 a2 = __float2half2_rn(0.f);
+        unsigned mo = 0u;
         if (lane < nf) {
             f0 = a_idx[p0 + lane];
             const float a = a_val[p0 + lane] * a_scale;
             a0 = Ops::left_weight(a);
             a2 = __half2half2(__float2half_ru(fabsf(a * b_scale)));   // rounded up: the bound must not fall short
+            mo = (unsigned)f0 * (unsigned)(Tp >> 2);
         }
         const int2 *drow = bdir + f0 * n_tiles;
         const int nk = nf < 32 ? nf : 32;
         // fp16 arithmetic of the bound: one rounding of at most 2^-11 (values below 2) per kept feature
         const float slack = 5e-4f * (float)nf + 1e-4f;
 
-        for (int tb0 = tb_begin; tb0 < t_end; tb0 += 64) {
+        for (int tb0 = tb_begin; tb0 < t_end; tb0 += 128) {
             int tb = tb0;
             if constexpr (FLOOR) {
-                tb += own_batch * 64;           // batches of the group in rotated order
-                if (tb >= t_end) tb -= (t_end - tb_begin + 63) / 64 * 64;
+                tb += own_pass * 128;           // passes of the group in rotated order
+                if (tb >= t_end) tb -= (t_end - tb_begin + 127) / 128 * 128;
                 const float f = __shfl_sync(FULL, __ldcg(fa.floor + row), 0);
                 if (f > floor_seen) {
                     floor_seen = f;
                     thr_r = fmaxf(thr_r, __fsub_rd(__fsub_rd(f, e_r), FLOOR_EPS));
                 }
             }
-            // ---- bounds of tiles tb + 2*lane and tb + 2*lane + 1 (tiles wholly below the rank are not taken)
-            unsigned m_even, m_odd;
-            const int t0 = tb + 2 * lane;
-            const bool up0 = (t0 + 1) * W > dr, up1 = (t0 + 2) * W > dr;
+            // ---- bounds of tiles t0 = tb + 4*lane .. t0 + 3 (tiles wholly below the rank are not taken).  A lane
+            // whose tiles all lie at or past t_end reads lane 0's maxima instead (the same sectors, so no extra
+            // traffic, and never past Tp) and passes none of them.
+            unsigned pass4;         // bit j: tile t0 + j passes
+            const int t0 = tb + 4 * lane;
             {
-                __half2 ub2 = __float2half2_rn(0.f);
-                const uint32_t *mrow = maxw_h + (tb >> 1) + lane;
-                // SG_FILTER_MLP block-maxima loads in flight per lane
-                for (int k0 = 0; k0 < nk; k0 += SG_FILTER_MLP) {
-                    uint32_t m[SG_FILTER_MLP];
-                    __half2 ak2[SG_FILTER_MLP];
-#pragma unroll
-                    for (int u = 0; u < SG_FILTER_MLP; ++u) {
-                        const int kk = k0 + u;
-                        const int fk = __shfl_sync(FULL, f0, kk & 31);
-                        ak2[u] = __shfl_sync(FULL, a2, kk & 31);
-                        m[u] = kk < nk ? mrow[fk * (Tp >> 1)] : 0u;
-                    }
-#pragma unroll
-                    for (int u = 0; u < SG_FILTER_MLP; ++u)
-                        ub2 = __hfma2(ak2[u], *reinterpret_cast<const __half2 *>(&m[u]), ub2);
+                const unsigned q = (unsigned)(tb >> 2) + (t0 < t_end ? lane : 0);   // + row offset: < 2^31
+                const uint2 *maxw4 = reinterpret_cast<const uint2 *>(maxw_h);
+                __half2 ub01 = __float2half2_rn(0.f), ub23 = __float2half2_rn(0.f);
+                for (int kk = 0; kk < nk; ++kk) {
+                    const unsigned o = __shfl_sync(FULL, mo, kk);
+                    const __half2 ak = __shfl_sync(FULL, a2, kk);
+                    const uint2 mv = maxw4[o + q];
+                    ub01 = __hfma2(ak, *reinterpret_cast<const __half2 *>(&mv.x), ub01);
+                    ub23 = __hfma2(ak, *reinterpret_cast<const __half2 *>(&mv.y), ub23);
                 }
                 // the kept features after the first 32, one chunk of 32 at a time
                 for (int base = 32; base < nf; base += 32) {
-                    int fl = 0;
+                    unsigned ol = 0u;
                     __half2 al = __float2half2_rn(0.f);
                     if (base + lane < nf) {
-                        fl = a_idx[p0 + base + lane];
+                        ol = (unsigned)a_idx[p0 + base + lane] * (unsigned)(Tp >> 2);
                         al = __half2half2(__float2half_ru(fabsf(a_val[p0 + base + lane] * a_scale * b_scale)));
                     }
                     const int nc = nf - base < 32 ? nf - base : 32;
                     for (int kk = 0; kk < nc; ++kk) {
-                        const int fk = __shfl_sync(FULL, fl, kk);
+                        const unsigned o = __shfl_sync(FULL, ol, kk);
                         const __half2 ak = __shfl_sync(FULL, al, kk);
-                        const uint32_t mv = mrow[fk * (Tp >> 1)];
-                        ub2 = __hfma2(ak, *reinterpret_cast<const __half2 *>(&mv), ub2);
+                        const uint2 mv = maxw4[o + q];
+                        ub01 = __hfma2(ak, *reinterpret_cast<const __half2 *>(&mv.x), ub01);
+                        ub23 = __hfma2(ak, *reinterpret_cast<const __half2 *>(&mv.y), ub23);
                     }
                 }
-                const float2 ub = __half22float2(ub2);
-                const float2 tb2 = reinterpret_cast<const float2 *>(tile_bound)[(tb >> 1) + lane];
-                const float thr0 = xp > 0.f ? fmaxf(fmaf(-xp, tb2.x, thr_r), 0.f) : thr_r;
-                const float thr1 = xp > 0.f ? fmaxf(fmaf(-xp, tb2.y, thr_r), 0.f) : thr_r;
-                m_even = __ballot_sync(FULL, t0 < t_end && up0 && ub.x + slack > thr0 * b_scale);
-                m_odd = __ballot_sync(FULL, t0 + 1 < t_end && up1 && ub.y + slack > thr1 * b_scale);
+                const float2 u01 = __half22float2(ub01), u23 = __half22float2(ub23);
+                const float4 tb4 = reinterpret_cast<const float4 *>(tile_bound)[q];
+                const float thr0 = xp > 0.f ? fmaxf(fmaf(-xp, tb4.x, thr_r), 0.f) : thr_r;
+                const float thr1 = xp > 0.f ? fmaxf(fmaf(-xp, tb4.y, thr_r), 0.f) : thr_r;
+                const float thr2 = xp > 0.f ? fmaxf(fmaf(-xp, tb4.z, thr_r), 0.f) : thr_r;
+                const float thr3 = xp > 0.f ? fmaxf(fmaf(-xp, tb4.w, thr_r), 0.f) : thr_r;
+                pass4 = (t0 < t_end && (t0 + 1) * W > dr && u01.x + slack > thr0 * b_scale ? 1u : 0u) |
+                        (t0 + 1 < t_end && (t0 + 2) * W > dr && u01.y + slack > thr1 * b_scale ? 2u : 0u) |
+                        (t0 + 2 < t_end && (t0 + 3) * W > dr && u23.x + slack > thr2 * b_scale ? 4u : 0u) |
+                        (t0 + 3 < t_end && (t0 + 4) * W > dr && u23.y + slack > thr3 * b_scale ? 8u : 0u);
             }
-            // ---- walk the surviving tiles; the directory entry of the next one is fetched ahead
-            int t = -1;
-            if (m_even) { t = tb + 2 * (__ffs(m_even) - 1); m_even &= m_even - 1; }
-            else if (m_odd) { t = tb + 2 * (__ffs(m_odd) - 1) + 1; m_odd &= m_odd - 1; }
+            // ---- walk the surviving tiles in increasing order; the directory entry of the next one is fetched
+            // ahead.  Each lane keeps only its own four bits (one register where warp-wide masks would take four).
+            auto next_tile = [&]() -> int {
+                const unsigned m = __ballot_sync(FULL, pass4 != 0u);
+                if (!m) return -1;
+                const int s = __ffs(m) - 1;
+                const int j = __ffs(__shfl_sync(FULL, pass4, s)) - 1;
+                if (lane == s) pass4 &= pass4 - 1u;
+                return tb + 4 * s + j;
+            };
+            int t = next_tile();
             int2 d_cur = make_int2(0, 0);
             if (t >= 0 && lane < nf) d_cur = drow[t];
             while (t >= 0) {
-                int t_next = -1;
-                if (m_even) { t_next = tb + 2 * (__ffs(m_even) - 1); m_even &= m_even - 1; }
-                else if (m_odd) { t_next = tb + 2 * (__ffs(m_odd) - 1) + 1; m_odd &= m_odd - 1; }
+                const int t_next = next_tile();
                 int2 d_next = make_int2(0, 0);
                 if (t_next >= 0 && lane < nf) d_next = drow[t_next];
 
