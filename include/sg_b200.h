@@ -370,6 +370,34 @@ int sg_cossim_candidates_range(const int64_t *a_indptr /*[dev]*/, const int32_t 
                                int32_t *cand_col /*[dev] cap*/, float *cand_partial /*[dev] cap or NULL*/,
                                int64_t cand_cap, unsigned long long *cand_count /*[dev] 1*/,
                                unsigned long long *row_queue /*[dev] 1*/, int warps_per_cta, void *stream);
+/*
+ * sg_cossim_candidates_range with the top-n floor of sg_cossim_candidates_floor (the keyed arg-max: 1 <= top_n <= 32,
+ * non-negative weights, warps_per_cta = 8, no triangle, so lo_pos is the start of the row's block).  Floors rise only
+ * from the pairs inside each row's range.  Self-match (`self_rank` [dev] per row id: the row's position in the blocked
+ * order of the right rows, which lies in [lo_pos, hi_pos) of the row): `flags` & SG_FLOOR_SEED walks only the
+ * column-tile group holding that position, from the 128-tile pass holding it, and leaves `group_items` untouched;
+ * without it every other group the range reaches.  self_rank = NULL: every group the range reaches.
+ */
+int sg_cossim_candidates_range_floor(const int64_t *a_indptr /*[dev]*/, const int32_t *a_len /*[dev] or NULL*/,
+                                     const int32_t *a_indices /*[dev]*/, const float *a_val32 /*[dev]*/,
+                                     int64_t row_begin, int64_t row_end, const int32_t *perm_a /*[dev] or NULL*/,
+                                     int64_t n_right, int64_t n_cols, const void *bucket_dir /*[dev]*/,
+                                     const void *bucket_maxw /*[dev]*/, const void *postings /*[dev]*/,
+                                     const int32_t *perm_b /*[dev] or NULL*/, int tile_w, int acc_dtype,
+                                     float a_scale, float b_scale, float cand_threshold,
+                                     const float *cand_threshold_row /*[dev] per row id, or NULL*/,
+                                     const float *pruned_norm_row /*[dev] per row id, or NULL*/,
+                                     const float *tile_bound /*[dev]*/, int64_t tiles_per_group,
+                                     const int32_t *lo_pos /*[dev] per left row id*/,
+                                     const int32_t *hi_pos /*[dev] per left row id*/,
+                                     unsigned long long *group_items /*[dev] scratch*/,
+                                     int32_t *cand_row /*[dev] cap*/, int32_t *cand_col /*[dev] cap*/,
+                                     float *cand_partial /*[dev] cap or NULL*/, int64_t cand_cap,
+                                     unsigned long long *cand_count /*[dev] 1*/,
+                                     unsigned long long *row_queue /*[dev] 1*/, int warps_per_cta,
+                                     float *row_floor /*[dev] per left row id*/, int top_n, float floor_margin,
+                                     float floor_margin_per_feature,
+                                     const int32_t *self_rank /*[dev] per row id, or NULL*/, int flags, void *stream);
 
 /* ------------------------------------------------------------------------- *
  * K2, tile-centric form (csrc/sg_tiles.cu) — the default for L2-normalised non-negative matrices (K1 output).

@@ -620,7 +620,7 @@ def prune_left_floor(A, B, hrank, row_begin, row_end, threshold, margin, margin_
 
 
 def cossim_nearest(A, B, threshold, stats=None, prune=None, acc=None, kernel=None, floor=None, tile_w=None,
-                   warps=None):
+                   warps=None, block_ids=None):
     """For every row i of A: the row j of B with the largest exact score A_i . B_j > threshold, the lowest j among
     equal scores (match_nearest, DESIGN.md §4 "Nearest row").  Returns host arrays (best int64 [n], -1 where no
     score passes; score float64 [n], 0 there).
@@ -628,17 +628,21 @@ def cossim_nearest(A, B, threshold, stats=None, prune=None, acc=None, kernel=Non
     Runs cossim_topn's path with top_n = 1 (pruning levels, row chunks, candidate-buffer retry, the top-n floor under
     `floor` / SG_B200_TOPN_FLOOR, the floor init without a threshold), but over the full product (no triangle, no
     dedup) and with the arg-max re-score (sg_rescore_nearest / sg_rescore_refined_nearest) instead of the top-n
-    selection: the selection keeps the larger column among equal scores, the arg-max the smaller one."""
+    selection: the selection keeps the larger column among equal scores, the arg-max the smaller one.
+
+    `block_ids` (cossim_topn's pair of int32 device tensors, one id per row of A and one per row of B): only the
+    rows j of B with row i's id compete, as in the blocked top-n product, the top-n floor included (DESIGN.md §4
+    "Blocks").  The same matrix on both sides may take two different tensors."""
     t = require_cuda()
     n = A.shape[0]
     if n == 0 or B.shape[0] == 0 or A.nnz == 0 or B.nnz == 0:
         if A.shape[1] != B.shape[1]:
             raise ValueError("dimension mismatch: left has %d features, right has %d" % (A.shape[1], B.shape[1]))
         if stats is not None:
-            stats.update(nearest=True, topn_floor=False, n_nearest_written=0)
+            stats.update(nearest=True, topn_floor=False, n_nearest_written=0, blocks=block_ids is not None)
         return np.full(n, -1, dtype=np.int64), np.zeros(n, dtype=np.float64)
     best, score = cossim_topn(A, B, 1, threshold, tile_w=tile_w, warps=warps, stats=stats, prune=prune, acc=acc,
-                              kernel=kernel, floor=floor, dedup=False, nearest=True)
+                              kernel=kernel, floor=floor, dedup=False, nearest=True, block_ids=block_ids)
     return tuple(to_host(best.to(t.int64), score))
 
 
@@ -692,8 +696,9 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
     self-match): only the pairs whose two rows have equal ids are eligible, and C[i,:] is the top_n of those (DESIGN.md
     §4 "Blocks").  Both sides run in the blocked processing order (block id, then the usual order), every left row
     reports the positions of its block among the right rows only (sg_cossim_candidates_range), and the scores are
-    those of the unblocked product bit for bit.  The top-n floor, the identical-rows dedup and the tile kernel are not
-    taken: floor=True, dedup=True and kernel="tiles" raise ValueError, SG_B200_KERNEL=tiles runs the row kernel.
+    those of the unblocked product bit for bit.  The identical-rows dedup and the tile kernel are not taken: dedup=True
+    and kernel="tiles" raise ValueError, SG_B200_KERNEL=tiles runs the row kernel.  The top-n floor runs with block ids
+    for `nearest` only (sg_cossim_candidates_range_floor); floor=True raises ValueError otherwise.
     """
     t = require_cuda()
     L = _lib.load()
@@ -715,21 +720,22 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
     blocked = block_ids is not None
     if blocked:
         ids_a, ids_b = block_ids
-        if nearest:
-            raise ValueError("cossim_nearest takes no block ids")
         for ids, n, side in ((ids_a, n_left, "left"), (ids_b, n_right, "right")):
             if ids.dtype != t.int32 or ids.dim() != 1 or ids.numel() != n or ids.device != dev:
                 raise ValueError("block ids of the %s matrix must be %d int32 values on %s" % (side, n, dev))
-        if (A is B) != (ids_a is ids_b):
+        # the arg-max has no triangle: one matrix on both sides may carry two different key columns
+        if (ids_a is ids_b and A is not B) or (A is B and ids_a is not ids_b and not nearest):
             raise ValueError("a self-match takes one block-id tensor for both sides, two matrices take two")
-        if floor is True:
+        if floor is True and not nearest:
             raise ValueError("the top-n floor does not run with block ids")
         if dedup is True:
             raise ValueError("the identical-rows dedup does not run with block ids")
         if kernel is not None and kernel.lower() == "tiles":
             raise ValueError("the tile kernel does not run with block ids")
         kernel = "row"
-        floor = dedup = False
+        dedup = False
+        if not nearest:
+            floor = False
     if n_rows == 0 or n_right == 0 or top_n <= 0 or A.nnz == 0 or B.nnz == 0:
         z32 = _empty(1, t.int32, dev)
         return DeviceMatches(shape, z32, z32, _empty(1, t.float64, dev), 0, 0)
@@ -742,6 +748,8 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
                          % (signed_margin, CAND_MARGIN, threshold))
     if stats is not None:
         stats["blocks"] = blocked
+        if blocked:
+            stats["n_blocks_used"] = int(t.unique(ids_a if ids_a is ids_b else t.cat([ids_a, ids_b])).numel())
 
     if floor not in (None, "auto", True, False):
         raise ValueError("floor must be None, 'auto', True or False, got %r" % (floor,))
@@ -756,7 +764,7 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
     row_best = t.zeros(n_rows, dtype=t.int64, device=dev) if nearest else None     # sg_rescore_nearest's running best
     if floor is True or (floor == "auto" and floor_ok and float(threshold) < 0.5 and n_rows >= FLOOR_MIN_ROWS):
         out = _cossim_topn_floor(A, B, top_n, float(threshold), row_begin, row_end, tile_w, stats, prune, acc,
-                                 decide=floor == "auto", row_best=row_best)
+                                 decide=floor == "auto", row_best=row_best, block_ids=block_ids)
         if out is not None:
             return out
     if stats is not None:
@@ -854,8 +862,6 @@ def cossim_topn(A, B, top_n, threshold, row_begin=0, row_end=None, tile_w=None, 
         # (left row, right row) pairs the launches visit, cumulated along perm_a: the density limit and row chunks
         pair_cum = np.zeros(n_rows + 1, dtype=np.int64)
         pair_cum[1:] = to_host(t.cumsum((hi_pos - diag_rank)[perm_a.long()].long(), 0))[0]
-        if stats is not None:
-            stats["n_blocks_used"] = int(t.unique(ids_a if triangle else t.cat([ids_a, ids_b])).numel())
     elif triangle:
         perm_a, diag_rank = perm_b, right_order(B)[2]
     else:
@@ -1156,7 +1162,7 @@ def row_keys(M, hrank, row_begin=0, row_end=None, row_norm=None, norm_scale=1.0)
     return keys ^ t.iinfo(t.int64).min
 
 
-def topn_floor_init(A, B, top_n, threshold, row_begin=0, row_end=None):
+def topn_floor_init(A, B, top_n, threshold, row_begin=0, row_end=None, blocks=None):
     """Initial top-n floors of rows [row_begin,row_end) of A against B (DESIGN.md §4): fp32 [A.shape[0]], zero
     outside the range.
 
@@ -1166,7 +1172,13 @@ def topn_floor_init(A, B, top_n, threshold, row_begin=0, row_end=None):
     the ends, so its columns are distinct.  sg_rescore scores the pairs exactly and keeps those above
     max(threshold, 0); the floor is the top_n-th best of them (sg_topn_select_rows), 0 for a row with fewer, written
     in fp32 rounded down.  It is the top_n-th best exact score of top_n distinct real pairs above the threshold, so it
-    never exceeds the row's exact top_n-th best."""
+    never exceeds the row's exact top_n-th best.
+
+    `blocks` (ids_a, ids_b, perm, rank, sorted_ids, lo, hi) of a blocked product (blocked_right_side, block_ranges):
+    the right order is the blocked one and row r's window holds min(FLOOR_INIT_WINDOW, hi[r] - lo[r]) right rows
+    inside [lo[r], hi[r]), around the insertion point of its key within its block (a self-match: its own position),
+    shifted inside the block; a row whose block has no right rows keeps floor 0.  Every pair of the window is eligible,
+    so the argument above holds."""
     t = require_cuda()
     L = _lib.load()
     row_end = A.shape[0] if row_end is None else int(row_end)
@@ -1178,17 +1190,41 @@ def topn_floor_init(A, B, top_n, threshold, row_begin=0, row_end=None):
     if n_rows <= 0 or K == 0 or top_n <= 0:
         return floor
     hrank, perm_b, rank_b = right_order(B)
-    if A is B:
+    if blocks is not None:
+        ids_a, ids_b, perm_b, rank_b, sorted_ids, lo, hi = blocks
+        lo, hi = lo[row_begin:row_end].long(), hi[row_begin:row_end].long()
+    if A is B and (blocks is None or ids_a is ids_b):
         pos = rank_b[row_begin:row_end].long()
     else:
         scale = 1.0 / max(B.norm_bound, 1e-30)        # the norm scale of right_order(B)
         keys_b = row_keys(B, hrank, row_norm=B._heavy_norm, norm_scale=scale)[perm_b.long()]
         keys_a = row_keys(A, hrank, row_begin, row_end, heavy_norms(A, hrank, row_begin, row_end), scale)
-        pos = t.searchsorted(keys_b, keys_a)
-    start = (pos - K // 2).clamp(0, n_right - K)
-    cand_col = perm_b[(start[:, None] + t.arange(K, device=dev)).reshape(-1)].contiguous()
-    cand_row = t.arange(row_begin, row_end, dtype=t.int32, device=dev).repeat_interleave(K)
-    n = n_rows * K
+        if blocks is None:
+            pos = t.searchsorted(keys_b, keys_a)
+        else:
+            # insertion point by (block id, key): the left keys first, so that a stable sort puts each before equal
+            # right keys (searchsorted's side); the right rows keep their blocked order
+            ka = t.cat([keys_a, keys_b])
+            o = t.sort(ka, stable=True).indices
+            o = o[t.sort(t.cat([ids_a[row_begin:row_end], sorted_ids])[o], stable=True).indices]
+            is_left = o < n_rows
+            rights_before = t.cumsum((~is_left).long(), 0) - (~is_left).long()
+            pos = t.empty(n_rows, dtype=t.int64, device=dev)
+            pos[o[is_left]] = rights_before[is_left]
+    if blocks is None:
+        start = (pos - K // 2).clamp(0, n_right - K)
+        cand_col = perm_b[(start[:, None] + t.arange(K, device=dev)).reshape(-1)].contiguous()
+        cand_row = t.arange(row_begin, row_end, dtype=t.int32, device=dev).repeat_interleave(K)
+    else:
+        k_r = (hi - lo).clamp(max=K)
+        start = t.minimum(t.maximum(pos - K // 2, lo), hi - k_r)
+        off = t.arange(K, device=dev)
+        valid = (off[None, :] < k_r[:, None]).reshape(-1)
+        cand_col = perm_b[(start[:, None] + off).reshape(-1)[valid]].contiguous()
+        cand_row = t.arange(row_begin, row_end, dtype=t.int32, device=dev).repeat_interleave(K)[valid].contiguous()
+    n = int(cand_row.numel())
+    if n == 0:
+        return floor
     score = _empty(n, t.float64, dev)
     keep_row, keep_col = _empty(n, t.int32, dev), _empty(n, t.int32, dev)
     count = t.zeros(1, dtype=t.int64, device=dev)
@@ -1222,7 +1258,8 @@ def topn_floor_init(A, B, top_n, threshold, row_begin=0, row_end=None):
     return floor
 
 
-def _cossim_topn_floor(A, B, top_n, threshold, row_begin, row_end, tile_w, stats, prune, acc, decide, row_best=None):
+def _cossim_topn_floor(A, B, top_n, threshold, row_begin, row_end, tile_w, stats, prune, acc, decide, row_best=None,
+                       block_ids=None):
     """cossim_topn with the top-n floor (DESIGN.md §4): row kernel, full product (no triangle), 8 warps per CTA.
 
     floor[r] is a proven lower bound of the exact score of row r's top_n-th best pair, raised by the candidates
@@ -1237,7 +1274,12 @@ def _cossim_topn_floor(A, B, top_n, threshold, row_begin, row_end, tile_w, stats
     without a threshold) are bounded by the block-max test like every other row.
 
     `row_best` (cossim_nearest, top_n = 1): the arg-max re-score with the floor replaces the top-n selection.  Every
-    pair scoring at least the floor is re-scored, so all pairs tied at a row's best are among them."""
+    pair scoring at least the floor is re-scored, so all pairs tied at a row's best are among them.
+
+    `block_ids` (cossim_topn's pair; only with `row_best`): both sides run in the blocked order, every launch is
+    sg_cossim_candidates_range_floor with the row's block [lo, hi) among the right rows (the decide sample the range
+    launch of the usual blocked path), the seed of a self-match starts at the row's blocked position, topn_floor_init
+    takes its windows inside the blocks, and row chunks are sized by the blocked pair count."""
     t = require_cuda()
     L = _lib.load()
     n_left, n_right = A.shape[0], B.shape[0]
@@ -1267,15 +1309,30 @@ def _cossim_topn_floor(A, B, top_n, threshold, row_begin, row_end, tile_w, stats
     tile_w, _ = pick_tile(n_right, tile_w, warps, 2 if acc == "u16" else 4, n_left=n_rows)
     while (-(-n_right // tile_w)) * (B.shape[1] + 1) > MAX_BUCKETS and tile_w < 32768:
         tile_w *= 2
-    hrank, perm_b, rank_b, bucket_dir, bucket_maxw, post, T, tile_bound = right_side(B, tile_w)
+    blocked = block_ids is not None
+    if blocked:
+        ids_a, ids_b = block_ids
+        hrank, perm_b, rank_b, bucket_dir, bucket_maxw, post, T, tile_bound, sorted_ids = \
+            blocked_right_side(B, ids_b, tile_w)
+        lo_pos, hi_pos = block_ranges(sorted_ids, ids_a)
+    else:
+        hrank, perm_b, rank_b, bucket_dir, bucket_maxw, post, T, tile_bound = right_side(B, tile_w)
     tiles_per_group = max(64, int(GROUP_BYTES // max(4 * B.nnz / T, 1)) // 64 * 64)
     # a self-match (any row range) seeds the floors from each row's own column-tile group
-    self_match = A is B
+    self_match = A is B and (not blocked or ids_a is ids_b)
     if self_match and row_begin == 0 and row_end == n_left:
         perm_a = perm_b
     else:
         perm_a, _ = row_order(A, hrank, row_begin, row_end, want_rank=False)
+        if blocked:
+            perm_a = blocked_order(perm_a, ids_a)
     self_rank = rank_b if self_match else None
+    group_items = pair_cum = None
+    if blocked:
+        group_items = _empty(2 * -(-T // tiles_per_group) + 1, t.int64, dev)
+        # (left row, right row) pairs of the rows along perm_a: the row chunks' share of the candidates
+        pair_cum = np.zeros(n_rows + 1, dtype=np.int64)
+        pair_cum[1:] = to_host(t.cumsum((hi_pos - lo_pos)[perm_a.long()].long(), 0))[0]
     total_mem = t.cuda.get_device_properties(dev).total_memory
     refine = REFINE and acc == "u16" and margin_pf > 0.0
     counters = t.zeros(4, dtype=t.int64, device=dev)   # [0] candidates / kept, [1] queue, [2] refined, [3] dropped
@@ -1305,11 +1362,19 @@ def _cossim_topn_floor(A, B, top_n, threshold, row_begin, row_end, tile_w, stats
         # the usual path's sample at its first pruning level (full product): its candidates at 24 B each
         l_idx, l_val, l_len, l_thr, l_xp, _ = arrays
         counters.zero_()
-        _lib.check(L.sg_cossim_candidates(
-            _ptr(A.d_indptr), _ptr(l_len), _ptr(l_idx), _ptr(l_val), row_begin, row_begin + int(sample.numel()),
-            _ptr(sample), n_right, A.shape[1], _ptr(bucket_dir), _ptr(bucket_maxw), _ptr(post), _ptr(perm_b), tile_w,
-            acc_code, a_scale, b_scale, thr_c, _ptr(l_thr), _ptr(l_xp), _ptr(tile_bound), tiles_per_group,
-            None, None, _ptr(dummy), _ptr(dummy), None, 0, c_count, c_queue, warps, _stream()))
+        if blocked:
+            _lib.check(L.sg_cossim_candidates_range(
+                _ptr(A.d_indptr), _ptr(l_len), _ptr(l_idx), _ptr(l_val), row_begin, row_begin + int(sample.numel()),
+                _ptr(sample), n_right, A.shape[1], _ptr(bucket_dir), _ptr(bucket_maxw), _ptr(post), _ptr(perm_b),
+                tile_w, acc_code, a_scale, b_scale, thr_c, _ptr(l_thr), _ptr(l_xp), _ptr(tile_bound), tiles_per_group,
+                _ptr(lo_pos), _ptr(hi_pos), _ptr(group_items), _ptr(dummy), _ptr(dummy), None, 0, c_count, c_queue,
+                warps, _stream()))
+        else:
+            _lib.check(L.sg_cossim_candidates(
+                _ptr(A.d_indptr), _ptr(l_len), _ptr(l_idx), _ptr(l_val), row_begin, row_begin + int(sample.numel()),
+                _ptr(sample), n_right, A.shape[1], _ptr(bucket_dir), _ptr(bucket_maxw), _ptr(post), _ptr(perm_b),
+                tile_w, acc_code, a_scale, b_scale, thr_c, _ptr(l_thr), _ptr(l_xp), _ptr(tile_bound), tiles_per_group,
+                None, None, _ptr(dummy), _ptr(dummy), None, 0, c_count, c_queue, warps, _stream()))
         LAUNCH_COUNTS["candidates"] += 1
         est_usual = int(counters[0].item()) * stride
         if stats is not None:
@@ -1319,7 +1384,8 @@ def _cossim_topn_floor(A, B, top_n, threshold, row_begin, row_end, tile_w, stats
     n_init_positive = None
     if no_threshold:
         # without a threshold every touched column is a candidate until a floor rises: start from proven floors
-        floor_buf = topn_floor_init(A, B, top_n, threshold, row_begin, row_end)
+        blocks = (ids_a, ids_b, perm_b, rank_b, sorted_ids, lo_pos, hi_pos) if blocked else None
+        floor_buf = topn_floor_init(A, B, top_n, threshold, row_begin, row_end, blocks)
         n_init_positive = int((floor_buf[row_begin:row_end] > 0).sum().item())
         arrays = pruned(floor_buf)
         mark(stats, "floor_init")
@@ -1329,6 +1395,16 @@ def _cossim_topn_floor(A, B, top_n, threshold, row_begin, row_end, tile_w, stats
     def launch(perm, n, arrs, row_buf, col_buf, part_buf, capacity, seed):
         l_idx, l_val, l_len, l_thr, l_xp, _ = arrs
         counters.zero_()
+        if blocked:
+            _lib.check(L.sg_cossim_candidates_range_floor(
+                _ptr(A.d_indptr), _ptr(l_len), _ptr(l_idx), _ptr(l_val), row_begin, row_begin + n, _ptr(perm),
+                n_right, A.shape[1], _ptr(bucket_dir), _ptr(bucket_maxw), _ptr(post), _ptr(perm_b), tile_w, acc_code,
+                a_scale, b_scale, thr_c, _ptr(l_thr), _ptr(l_xp), _ptr(tile_bound), tiles_per_group, _ptr(lo_pos),
+                _ptr(hi_pos), _ptr(group_items), _ptr(row_buf), _ptr(col_buf), _ptr(part_buf), capacity, c_count,
+                c_queue, warps, _ptr(floor_buf), top_n, margin, margin_pf, _ptr(self_rank),
+                _lib.SG_FLOOR_SEED if seed else 0, _stream()))
+            LAUNCH_COUNTS["candidates"] += 1
+            return int(counters[0].item())
         _lib.check(L.sg_cossim_candidates_floor(
             _ptr(A.d_indptr), _ptr(l_len), _ptr(l_idx), _ptr(l_val), row_begin, row_begin + n, _ptr(perm), n_right,
             A.shape[1], _ptr(bucket_dir), _ptr(bucket_maxw), _ptr(post), _ptr(perm_b), tile_w, acc_code,
@@ -1429,8 +1505,8 @@ def _cossim_topn_floor(A, B, top_n, threshold, row_begin, row_end, tile_w, stats
             cand, first = first, None
         else:
             perm_chunk = perm_a if (lo == 0 and hi == n_rows) else perm_a[lo:hi]
-            cap = base_cap if est is None else min(max(int(1.3 * est * (hi - lo) / n_rows) + (1 << 22), 1 << 22),
-                                                   1 << 31)
+            part = (hi - lo) / n_rows if pair_cum is None else (pair_cum[hi] - pair_cum[lo]) / max(pair_cum[-1], 1)
+            cap = base_cap if est is None else min(max(int(1.3 * est * part) + (1 << 22), 1 << 22), 1 << 31)
             cand = collect(perm_chunk, hi - lo, arrays, False, cap)
         n_main += cand[3]
         kept.append(rescore(cand, arrays))
@@ -1452,7 +1528,8 @@ def _cossim_topn_floor(A, B, top_n, threshold, row_begin, row_end, tile_w, stats
         stats["topn_floor"] = True
         stats["floor_init"] = no_threshold
         if no_threshold:
-            stats["n_candidates_init"] = n_rows * min(FLOOR_INIT_WINDOW, n_right)     # pairs scored by the init
+            stats["n_candidates_init"] = (int((hi_pos - lo_pos)[perm_a.long()].clamp(max=FLOOR_INIT_WINDOW).sum())
+                                          if blocked else n_rows * min(FLOOR_INIT_WINDOW, n_right))  # pairs the init scored
             stats["n_floor_init_positive"] = n_init_positive
             l_len = arrays[2]
             kept = (l_len[row_begin:row_end] if l_len is not None else

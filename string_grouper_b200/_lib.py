@@ -76,6 +76,9 @@ SIGNATURES = {
     "sg_cossim_candidates_range": (_i32, [_p, _p, _p, _p, _i64, _i64, _p, _i64, _i64, _p, _p, _p, _p, _i32, _i32,
                                           _f32, _f32, _f32, _p, _p, _p, _i64, _p, _p, _p, _p, _p, _p, _i64, _p, _p, _i32,
                                           _p]),
+    "sg_cossim_candidates_range_floor": (_i32, [_p, _p, _p, _p, _i64, _i64, _p, _i64, _i64, _p, _p, _p, _p, _i32,
+                                                _i32, _f32, _f32, _f32, _p, _p, _p, _i64, _p, _p, _p, _p, _p, _p, _i64,
+                                                _p, _p, _i32, _p, _i32, _f32, _f32, _p, _i32, _p]),
     "sg_tiles_tile_w": (_i32, []),
     "sg_tiles_max_cols": (_i64, []),
     "sg_tiles_blob_bound": (_i64, [_i64, _i64, _i64]),

@@ -389,6 +389,10 @@ __device__ __forceinline__ void apply_buckets(AccT *__restrict__ acc, const uint
 // Self-match (`self_rank` = every row's position in the common processing order): `seed` = 1 walks only the row's own
 // column-tile group, starting at the 128-tile pass that holds the row (clusters of identical names sit next to each
 // other in that order, so this is where floors rise first); `seed` = 0 walks every other group.
+// Both (cossim_candidates_range_floor_kernel, a keyed arg-max): the floor is raised only from pairs inside the row's
+// range, which the sweep's lo / hi cut has already masked, so it stays a bound of eligible pairs.  A self-match's seed
+// takes no group_items (one item per row, in the group holding self_rank[row], which lies in [lo, hi)); without the
+// seed the items come from group_items as for the range alone, and the row's own group is skipped.
 //
 // Long rows (more than 32 kept features: long records rows, names without a threshold): only the first 32 stay in
 // registers, but ub(t) is taken over ALL kept features, the later ones 32 at a time, their {row offset, weight} loaded
@@ -459,7 +463,9 @@ candidates_body(const int64_t *__restrict__ a_indptr, const int32_t *__restrict_
     const int64_t n_groups = (T + tiles_per_group - 1) / tiles_per_group;
     unsigned long long n_items =
         group_items ? group_items[n_groups] : (unsigned long long)n_rows * (unsigned long long)n_groups;
-    if constexpr (FLOOR) {
+    if constexpr (FLOOR && RANGE) {
+        if (fa.seed) n_items = (unsigned long long)n_rows;      // the seed takes no group_items: one item per row
+    } else if constexpr (FLOOR) {
         if (fa.self_rank) n_items = (unsigned long long)n_rows * (unsigned long long)(fa.seed ? 1 : n_groups - 1);
     }
     const int n_tiles = (int)T;
@@ -487,6 +493,8 @@ candidates_body(const int64_t *__restrict__ a_indptr, const int32_t *__restrict_
                 if (fa.seed) {
                     group = (int)own;
                     own_pass = (int)((pos / W - own * tiles_per_group) >> 7);
+                } else if constexpr (RANGE) {
+                    if (group == own) continue;     // group_items hand out the own group too: the seed walked it
                 } else if (group >= own) {
                     ++group;
                 }
@@ -513,6 +521,11 @@ candidates_body(const int64_t *__restrict__ a_indptr, const int32_t *__restrict_
         }
         const int t_first = (int)(((int64_t)dr / W) & ~127);           // the 128-tile pass holding the rank
         const int tb_begin = t_first > t_begin ? t_first : t_begin;
+        if constexpr (FLOOR && RANGE) {
+            // the passes start at tb_begin, which lo may have moved past the group's first tile; the row's own
+            // position lies in [lo, hi) and in its group, so its pass is one of them
+            if (fa.seed) own_pass = (int)(((int64_t)fa.self_rank[row] / W - tb_begin) >> 7);
+        }
 
         // the first 32 features of the row stay in registers; lane k also holds where its feature's block maxima row
         // starts, in 4-tile (8-byte) units: below T * V1 < 2^31 (checked by sg_postings_build), so 32 bits
@@ -724,6 +737,12 @@ template <int NW, typename AccT>
 __global__ void __launch_bounds__(NW * 32, min_ctas(NW))
     cossim_candidates_range_kernel(SG_CAND_PARAMS, const int32_t *__restrict__ hi_pos) {
     candidates_body<NW, AccT, false, true>(SG_CAND_ARGS, FloorArgs{}, hi_pos);
+}
+
+template <int NW, typename AccT>
+__global__ void __launch_bounds__(NW * 32, min_ctas(NW))
+    cossim_candidates_range_floor_kernel(SG_CAND_PARAMS, FloorArgs fa, const int32_t *__restrict__ hi_pos) {
+    candidates_body<NW, AccT, true, true>(SG_CAND_ARGS, fa, hi_pos);
 }
 #undef SG_CAND_PARAMS
 #undef SG_CAND_ARGS
@@ -1423,21 +1442,25 @@ static int launch_candidates(const int64_t *a_indptr, const int32_t *a_len, cons
                              int n_sm, cudaStream_t st, const FloorArgs &fa, const int32_t *hi_pos = nullptr) {
     const size_t smem = (size_t)NW * tile_w * sizeof(AccT);
     const void *kern;
-    if constexpr (RANGE) kern = (const void *)cossim_candidates_range_kernel<NW, AccT>;
+    if constexpr (RANGE && FLOOR) kern = (const void *)cossim_candidates_range_floor_kernel<NW, AccT>;
+    else if constexpr (RANGE) kern = (const void *)cossim_candidates_range_kernel<NW, AccT>;
     else if constexpr (FLOOR) kern = (const void *)cossim_candidates_floor_kernel<NW, AccT>;
     else kern = (const void *)cossim_candidates_kernel<NW, AccT>;
     SG_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const int64_t T = sg_num_tiles(n_right, tile_w);
     const int64_t n_rows = row_end - row_begin;
+    // the seed of a keyed floor launch hands out one item per row without group_items (candidates_body)
+    const bool items = !(RANGE && FLOOR && fa.seed);
     if constexpr (RANGE) {
-        const int64_t n_groups = (T + tiles_per_group - 1) / tiles_per_group;
-        SG_CUDA_TRY(cudaMemsetAsync(group_items, 0, (size_t)(2 * n_groups + 1) * sizeof(unsigned long long), st));
-        range_groups_kernel<<<(unsigned)((n_rows + 255) / 256), 256, 0, st>>>(n_rows, perm_a, row_begin, diag_rank,
-                                                                              hi_pos, tiles_per_group * tile_w,
-                                                                              n_groups, group_items);
-        SG_LAUNCH_CHECK();
-        range_items_kernel<<<1, 32, 0, st>>>(n_rows, n_groups, group_items);
-        SG_LAUNCH_CHECK();
+        if (items) {
+            const int64_t n_groups = (T + tiles_per_group - 1) / tiles_per_group;
+            SG_CUDA_TRY(cudaMemsetAsync(group_items, 0, (size_t)(2 * n_groups + 1) * sizeof(unsigned long long), st));
+            range_groups_kernel<<<(unsigned)((n_rows + 255) / 256), 256, 0, st>>>(
+                n_rows, perm_a, row_begin, diag_rank, hi_pos, tiles_per_group * tile_w, n_groups, group_items);
+            SG_LAUNCH_CHECK();
+            range_items_kernel<<<1, 32, 0, st>>>(n_rows, n_groups, group_items);
+            SG_LAUNCH_CHECK();
+        }
     } else if (diag_rank) {
         const int64_t n_groups = (T + tiles_per_group - 1) / tiles_per_group;
         SG_CUDA_TRY(cudaMemsetAsync(group_items, 0, (size_t)(n_groups + 1) * sizeof(unsigned long long), st));
@@ -1457,9 +1480,11 @@ static int launch_candidates(const int64_t *a_indptr, const int32_t *a_len, cons
     a_indptr, a_len, a_indices, a_val32, row_begin, row_end, perm_a, n_right, (const int2 *)bucket_dir,               \
         (const uint32_t *)bucket_maxw, (const uint32_t *)postings, perm_b, (int)sg_num_tiles_padded(n_right, tile_w), \
         tile_w, T, tiles_per_group, a_scale, b_scale, thr_c, thr_row, xp_norm, tile_bound, diag_rank,                \
-        diag_rank ? group_items : nullptr, cand_row, cand_col, cand_partial, (unsigned long long)cand_cap, cand_count, \
-        row_queue
-    if constexpr (RANGE)
+        diag_rank && items ? group_items : nullptr, cand_row, cand_col, cand_partial, (unsigned long long)cand_cap,  \
+        cand_count, row_queue
+    if constexpr (RANGE && FLOOR)
+        cossim_candidates_range_floor_kernel<NW, AccT><<<(unsigned)ctas, NW * 32, smem, st>>>(SG_KARGS, fa, hi_pos);
+    else if constexpr (RANGE)
         cossim_candidates_range_kernel<NW, AccT><<<(unsigned)ctas, NW * 32, smem, st>>>(SG_KARGS, hi_pos);
     else if constexpr (FLOOR)
         cossim_candidates_floor_kernel<NW, AccT><<<(unsigned)ctas, NW * 32, smem, st>>>(SG_KARGS, fa);
@@ -1470,7 +1495,8 @@ static int launch_candidates(const int64_t *a_indptr, const int32_t *a_len, cons
     return SG_OK;
 }
 
-// fa == NULL: cossim_candidates_kernel, or with `hi_pos` the position-range variant; otherwise the floor variant
+// fa == NULL: cossim_candidates_kernel, or with `hi_pos` the position-range variant; otherwise the floor variant,
+// with `hi_pos` the floor over a position range
 static int cossim_candidates(const int64_t *a_indptr, const int32_t *a_len, const int32_t *a_indices,
                              const float *a_val32, int64_t row_begin, int64_t row_end, const int32_t *perm_a,
                              int64_t n_right, int64_t n_cols, const void *bucket_dir, const void *bucket_maxw,
@@ -1511,6 +1537,9 @@ static int cossim_candidates(const int64_t *a_indptr, const int32_t *a_len, cons
         // the range variant is built for the default 8 warps only
         if (warps_per_cta != 8) return fail(SG_ERR_INVALID, "the position-range variant runs with 8 warps per CTA");
         if (!diag_rank || !group_items) return fail(SG_ERR_INVALID, "the position range needs lo_pos and group_items");
+        if (fa)
+            return acc_dtype == SG_ACC_U16 ? launch_candidates<8, uint16_t, true, true>(SG_ARGS, *fa, hi_pos)
+                                           : launch_candidates<8, float, true, true>(SG_ARGS, *fa, hi_pos);
         return acc_dtype == SG_ACC_U16 ? launch_candidates<8, uint16_t, false, true>(SG_ARGS, FloorArgs{}, hi_pos)
                                        : launch_candidates<8, float, false, true>(SG_ARGS, FloorArgs{}, hi_pos);
     }
@@ -1535,6 +1564,21 @@ static int cossim_candidates(const int64_t *a_indptr, const int32_t *a_len, cons
     }
 #undef SG_CASE
 #undef SG_ARGS
+}
+
+// FloorArgs of sg_cossim_candidates_floor and sg_cossim_candidates_range_floor from their arguments, checked
+static int floor_args(FloorArgs &fa, float *row_floor, int top_n, float floor_margin, float floor_margin_per_feature,
+                      const int32_t *self_rank, const int32_t *perm_a, int flags) {
+    if (!row_floor) return fail(SG_ERR_INVALID, "row_floor is required");
+    if (flags & ~(SG_FLOOR_SEED | SG_FLOOR_LONG_ROWS)) return fail(SG_ERR_INVALID, "unknown flags %d", flags);
+    const bool seed = (flags & SG_FLOOR_SEED) != 0;
+    if (top_n < 1 || top_n > 32) return fail(SG_ERR_INVALID, "the top-n floor supports 1 <= top_n <= 32, got %d", top_n);
+    if (!(floor_margin >= 0.f) || !(floor_margin_per_feature >= 0.f))
+        return fail(SG_ERR_INVALID, "floor margins must be >= 0");
+    if (seed && !self_rank) return fail(SG_ERR_INVALID, "seed needs self_rank");
+    if (self_rank && !perm_a) return fail(SG_ERR_INVALID, "self_rank needs perm_a");
+    fa = FloorArgs{row_floor, self_rank, seed ? 1 : 0, top_n, floor_margin, floor_margin_per_feature};
+    return SG_OK;
 }
 
 extern "C" {
@@ -1568,15 +1612,9 @@ int sg_cossim_candidates_floor(const int64_t *a_indptr, const int32_t *a_len, co
                                unsigned long long *cand_count, unsigned long long *row_queue, int warps_per_cta,
                                float *row_floor, int top_n, float floor_margin, float floor_margin_per_feature,
                                const int32_t *self_rank, int flags, void *stream_) {
-    if (!row_floor) return fail(SG_ERR_INVALID, "row_floor is required");
-    if (flags & ~(SG_FLOOR_SEED | SG_FLOOR_LONG_ROWS)) return fail(SG_ERR_INVALID, "unknown flags %d", flags);
-    const bool seed = (flags & SG_FLOOR_SEED) != 0;
-    if (top_n < 1 || top_n > 32) return fail(SG_ERR_INVALID, "the top-n floor supports 1 <= top_n <= 32, got %d", top_n);
-    if (!(floor_margin >= 0.f) || !(floor_margin_per_feature >= 0.f))
-        return fail(SG_ERR_INVALID, "floor margins must be >= 0");
-    if (seed && !self_rank) return fail(SG_ERR_INVALID, "seed needs self_rank");
-    if (self_rank && !perm_a) return fail(SG_ERR_INVALID, "self_rank needs perm_a");
-    const FloorArgs fa{row_floor, self_rank, seed ? 1 : 0, top_n, floor_margin, floor_margin_per_feature};
+    FloorArgs fa{};
+    const int rc = floor_args(fa, row_floor, top_n, floor_margin, floor_margin_per_feature, self_rank, perm_a, flags);
+    if (rc != SG_OK) return rc;
     return cossim_candidates(a_indptr, a_len, a_indices, a_val32, row_begin, row_end, perm_a, n_right, n_cols,
                              bucket_dir, bucket_maxw, postings, perm_b, tile_w, acc_dtype, a_scale, b_scale,
                              cand_threshold, cand_threshold_row, pruned_norm_row, tile_bound, tiles_per_group,
@@ -1603,6 +1641,30 @@ int sg_cossim_candidates_range(const int64_t *a_indptr, const int32_t *a_len, co
                              lo_pos, group_items,
                              cand_row, cand_col, cand_partial, cand_cap, cand_count, row_queue, warps_per_cta, stream_,
                              nullptr, hi_pos);
+}
+
+int sg_cossim_candidates_range_floor(const int64_t *a_indptr, const int32_t *a_len, const int32_t *a_indices,
+                                     const float *a_val32, int64_t row_begin, int64_t row_end, const int32_t *perm_a,
+                                     int64_t n_right, int64_t n_cols, const void *bucket_dir, const void *bucket_maxw,
+                                     const void *postings, const int32_t *perm_b, int tile_w, int acc_dtype,
+                                     float a_scale, float b_scale, float cand_threshold,
+                                     const float *cand_threshold_row, const float *pruned_norm_row,
+                                     const float *tile_bound, int64_t tiles_per_group, const int32_t *lo_pos,
+                                     const int32_t *hi_pos, unsigned long long *group_items, int32_t *cand_row,
+                                     int32_t *cand_col, float *cand_partial, int64_t cand_cap,
+                                     unsigned long long *cand_count, unsigned long long *row_queue, int warps_per_cta,
+                                     float *row_floor, int top_n, float floor_margin, float floor_margin_per_feature,
+                                     const int32_t *self_rank, int flags, void *stream_) {
+    if (!lo_pos || !hi_pos || !group_items) return fail(SG_ERR_INVALID, "lo_pos, hi_pos and group_items are required");
+    FloorArgs fa{};
+    const int rc = floor_args(fa, row_floor, top_n, floor_margin, floor_margin_per_feature, self_rank, perm_a, flags);
+    if (rc != SG_OK) return rc;
+    return cossim_candidates(a_indptr, a_len, a_indices, a_val32, row_begin, row_end, perm_a, n_right, n_cols,
+                             bucket_dir, bucket_maxw, postings, perm_b, tile_w, acc_dtype, a_scale, b_scale,
+                             cand_threshold, cand_threshold_row, pruned_norm_row, tile_bound, tiles_per_group,
+                             lo_pos, group_items,
+                             cand_row, cand_col, cand_partial, cand_cap, cand_count, row_queue, warps_per_cta, stream_,
+                             &fa, hi_pos);
 }
 
 }  // extern "C"

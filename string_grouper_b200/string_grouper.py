@@ -128,7 +128,8 @@ def match_most_similar(master: pd.Series, duplicates: pd.Series, master_id: Opti
 
 
 def match_nearest(master: pd.Series, duplicates: pd.Series, master_id: Optional[pd.Series] = None,
-                  duplicates_id: Optional[pd.Series] = None, **kwargs) -> Union[pd.DataFrame, pd.Series]:
+                  duplicates_id: Optional[pd.Series] = None, *, master_keys: Optional[pd.Series] = None,
+                  duplicates_keys: Optional[pd.Series] = None, **kwargs) -> Union[pd.DataFrame, pd.Series]:
     """For each string in duplicates the most similar string in master, as the reference documents
     match_most_similar (ref:100-108): the master with the largest similarity above min_similarity (min_similarity
     <= 0: above 0), the lowest master position among equal similarities, the duplicate itself where no master
@@ -137,9 +138,12 @@ def match_nearest(master: pd.Series, duplicates: pd.Series, master_id: Optional[
     match_most_similar keeps the reference's code instead, which keeps one duplicate per master: a duplicate whose
     best master already holds a better-scoring duplicate comes back unmatched or with a worse master.  match_nearest
     equals `StringGrouper(master, duplicates, ..., max_n_matches=len(duplicates)).fit().get_groups()` without
-    materialising every pair above the threshold."""
+    materialising every pair above the threshold.
+
+    With blocking keys (see StringGrouper; give both or neither) only the masters of the duplicate's own key compete;
+    a duplicate whose key no master has (or whose key is missing) comes back as itself, like an unmatched one."""
     return StringGrouper(master, duplicates=duplicates, master_id=master_id, duplicates_id=duplicates_id,
-                         **kwargs)._match_nearest()
+                         master_keys=master_keys, duplicates_keys=duplicates_keys, **kwargs)._match_nearest()
 
 
 def match_strings(master: pd.Series, duplicates: Optional[pd.Series] = None, master_id: Optional[pd.Series] = None,
@@ -371,7 +375,7 @@ class StringGrouper(object):
         rank, world_size = _dist.world()
         if self._block_ids is not None:
             # blocking keys: only pairs of equal block ids (the vectoriser and the scores are the unkeyed ones)
-            block_ids = _device.block_id_tensors(self._block_ids, A.shape[0], B is A)
+            block_ids = self._block_id_tensors(A.shape[0], B is A)
             out = _device.cossim_topn(A, B, self._max_n_matches, self._config.min_similarity,
                                       stats=self._last_stats, block_ids=block_ids)
         elif world_size > 1 and getattr(A, "row_offset", None) is not None:
@@ -494,9 +498,11 @@ class StringGrouper(object):
         self.update_options(**kwargs)
         return self.fit().get_groups()
 
-    def match_nearest(self, master, duplicates, master_id=None, duplicates_id=None, **kwargs):
+    def match_nearest(self, master, duplicates, master_id=None, duplicates_id=None, *, master_keys=None,
+                      duplicates_keys=None, **kwargs):
         """The module-level match_nearest on new data with these options merged with `kwargs`."""
-        self.reset_data(master, duplicates, master_id, duplicates_id)
+        self.reset_data(master, duplicates, master_id, duplicates_id, master_keys=master_keys,
+                        duplicates_keys=duplicates_keys)
         self.update_options(**kwargs)
         return self._match_nearest()
 
@@ -584,8 +590,19 @@ class StringGrouper(object):
         master_matrix, duplicate_matrix = self._get_tf_idf_matrices(shard=False)
         B = _device.as_device_csr(master_matrix)
         A = _device.as_device_csr(duplicate_matrix)
-        best, _ = _device.cossim_nearest(A, B, self._config.min_similarity, stats=self._last_stats)
+        block_ids = None
+        if self._block_ids is not None:
+            # the duplicates are the left operand: (duplicate ids, master ids)
+            ids_m, ids_d = self._block_id_tensors(len(self._master), False)
+            block_ids = (ids_d, ids_m)
+        best, _ = _device.cossim_nearest(A, B, self._config.min_similarity, stats=self._last_stats,
+                                         block_ids=block_ids)
         return self._nearest_frame(best, self._config.ignore_index, self._config.replace_na)
+
+    def _block_id_tensors(self, n_left, self_match):
+        """cossim_topn's block_ids pair from the ids of master ++ duplicates: (master ids, duplicate ids), or one
+        tensor twice for a self-match."""
+        return _device.block_id_tensors(self._block_ids, n_left, self_match)
 
     def _nearest_frame(self, best, ignore_index, replace_na) -> Union[pd.DataFrame, pd.Series]:
         """The result frame of _get_nearest_matches from best[d] = master position of duplicate d (-1: none)."""
@@ -829,17 +846,27 @@ def block_ids_of(master, duplicates=None, master_keys=None, duplicates_keys=None
     sides = [(master, master_keys, 'master')] + ([] if duplicates is None else [(duplicates, duplicates_keys,
                                                                                   'duplicates')])
     for strings, keys, name in sides:
-        if not isinstance(keys, pd.Series):
-            raise TypeError(f'{name}_keys must be a pandas.Series')
-        if len(keys) != len(strings):
-            raise ValueError(f'{name}_keys has {len(keys)} values for {len(strings)} strings')
-    keys = pd.concat([k for _, k, _ in sides], ignore_index=True)
+        check_keys(strings, keys, f'{name}_keys')
+    return factorise_keys(pd.concat([k for _, k, _ in sides], ignore_index=True))[0]
+
+
+def check_keys(strings, keys, label):
+    """TypeError / ValueError unless `keys` is a Series with one value per string."""
+    if not isinstance(keys, pd.Series):
+        raise TypeError(f'{label} must be a pandas.Series')
+    if len(keys) != len(strings):
+        raise ValueError(f'{label} has {len(keys)} values for {len(strings)} strings')
+
+
+def factorise_keys(keys, first_id=0):
+    """(int32 id per key, the distinct present values in id order): equal values get equal ids from first_id on, in
+    order of appearance, and every missing value (None, NaN, pd.NA) an id of its own after them."""
     codes, uniques = pd.factorize(keys, use_na_sentinel=True)
     missing = codes < 0
     codes[missing] = len(uniques) + np.arange(int(missing.sum()))
-    if len(uniques) + int(missing.sum()) >= 2**31:
+    if first_id + len(uniques) + int(missing.sum()) >= 2**31:
         raise OverflowError('more than 2^31 - 1 distinct blocking keys')
-    return codes.astype(np.int32)
+    return (codes + first_id).astype(np.int32), uniques
 
 
 def _is_arrow_str(series):
